@@ -1,8 +1,9 @@
 #!/usr/bin/env python
 """Benchmark of the OctFusion denoising U-Net hot path (BASELINE.json: "U-Net denoise steps/sec
-(depth-6, B=32) at 1/2/4/8 B200").
+(depth-6, B=32) at 1/2/4/8 H100").
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--workload unet|cond|vae]
+                    [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
 
 A step = one pass of the hot path over one batch: the stage-2 ("hr") U-Net forward on B=32 synthetic depth-6
@@ -15,15 +16,18 @@ One JSON line on stdout (rank 0):
   value        whole-job steps/s, inputs resident in HBM (CUDA-graph replay, CUDA events, max over ranks)
   e2e          the same metric through the public sampler API (HRStepper) with the latent arriving from pinned host
                memory and the result returning to the host every step (copies inside the timed region)
-  roofline     the tcgen05 tap-gather GEMM aggregated over all its launches of one step (per-launch CUDA events)
-  cpu_baseline the reference's own modules (build container) or the oracle port (GPU box: the reference tree does
-               not travel) on the host cores: bounded sample, thread-count sweep, best reported
-  library_baseline  the reference op sequence (oracle port = the same ATen calls) on the SAME B200 in fp32 through
+  roofline     the tensor-core tap-gather GEMM aggregated over all its launches of one step (per-launch CUDA events)
+  cpu_baseline the oracle port of the reference path (oracle/restate.py: the reference's ATen op sequence, pinned against
+               the reference by tests/golden/) on the host cores: bounded sample, thread-count sweep, best reported
+  library_baseline  the reference op sequence (oracle port = the same ATen calls) on the SAME GPU in fp32 through
                ATen / cuBLAS -- the "same-box library" bar of BASELINE.md section 3
 Multi-GPU (BASELINE.json configs[2]): the B=32 shapes are SHARDED over the ranks (32/N per GPU, `scaling: strong`);
 no collective in the step loop (SURVEY.md 8e); one ragged all-gather of the final latents after the timed region.
 `--weak` keeps 32 shapes per GPU instead.  --workload cond = the class-conditional config (configs[4]);
 --workload vae = GraphVAE encode + decode at depth 8 (configs[3], HBM-bound regime).
+--dump-outputs DIR writes what the timed path computed in its last timed step as DIR/<name>.npy (float32): unet / cond
+the denoised latent and the predicted noise, vae the decoder outputs.  The inputs are seeded, so two builds run with
+the same arguments can be compared output for output.
 """
 from __future__ import annotations
 import argparse
@@ -49,6 +53,9 @@ COND = dict(UNCOND, num_res_blocks=[[1, 1, 1], [2, 2, 0]], attention_resolutions
 METRICS = {'unet': 'unet_denoise_steps_per_sec_depth6_B32', 'cond': 'unet_cond_denoise_steps_per_sec_depth6_B32',
            'vae': 'graphvae_encode_decode_per_sec_depth8'}
 UNIT = 'steps/s'
+# NVIDIA H100 SXM data sheet (dense, 700 W card): the denominators of the roofline fractions when no measured peak is given
+H100_BF16_TFLOPS = 989.0
+H100_HBM_GBS = 3350.0
 
 
 def parse():
@@ -66,7 +73,33 @@ def parse():
     ap.add_argument('--no-cpu-baseline', action='store_true')
     ap.add_argument('--no-library-baseline', action='store_true')
     ap.add_argument('--no-roofline', action='store_true')
-    return ap.parse_args()
+    ap.add_argument('--dump-outputs', metavar='DIR', default=None,
+                    help='write the outputs of the last timed step to DIR/<name>.npy (float32, <= 64 MB in all)')
+    args = ap.parse_args()
+    if args.steps < 1 or args.warmup < 0:
+        ap.error('--steps must be >= 1 and --warmup >= 0')
+    return args
+
+
+DUMP_BYTES = 64 << 20
+
+
+def dump_outputs(out_dir, arrays):
+    """arrays: name -> tensor of the last timed step.  Each tensor is flattened to [rows, -1] float32; when the whole set
+    exceeds DUMP_BYTES the same fixed, seeded sample of rows is kept of every tensor with that row count, and the
+    sampled row indices are written beside them as <name>_rows.npy (float64)."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    flat = {k: v.detach().float().reshape(v.shape[0], -1).cpu() for k, v in arrays.items()}
+    total = sum(v.numel() * 4 for v in flat.values())
+    sampled = sum(v.shape[0] * (v.shape[1] * 4 + 8) for v in flat.values())     # values + float64 row index
+    for name, v in flat.items():
+        if total > DUMP_BYTES:
+            keep = max(1, int(v.shape[0] * (DUMP_BYTES - 4096 * len(flat)) // sampled))
+            rows = torch.randperm(v.shape[0], generator=torch.Generator().manual_seed(0))[:keep].sort().values
+            v = v[rows]
+            np.save(os.path.join(out_dir, name + '_rows.npy'), rows.numpy().astype(np.float64))
+        np.save(os.path.join(out_dir, name + '.npy'), v.numpy().astype(np.float32))
 
 
 def config_for(args):
@@ -186,12 +219,11 @@ def _move_graph(dg, dev):
     return g2
 
 
-def baseline_step_fn(cfg, cfg_name, batch, device, use_reference):
+def baseline_step_fn(cfg, cfg_name, batch, device):
     """returns (step callable, kind): one U-Net forward + eps-DDIM update on `batch` of the synthetic shapes in fp32,
-    by the unmodified reference modules (when /root/reference is present and device is the CPU) or the oracle port."""
+    by the oracle port of the reference path (the benchmark never imports the reference tree)."""
     from oracle import restate as R
     from oracle.octree_util import octree_from_splits
-    from oracle import ref_import
     l4, l5 = _synth().synth_splits(batch, 0)
     octree = octree_from_splits(l4, l5, batch)
     cc = cfg['input_channels'][1]
@@ -199,19 +231,6 @@ def baseline_step_fn(cfg, cfg_name, batch, device, use_reference):
     ts = torch.full((batch,), 1.5)
     label = (torch.arange(batch) % cfg['num_classes']) if cfg.get('num_classes') else None
     ls, lsn = torch.tensor(1.5), torch.tensor(1.9)
-    if use_reference and ref_import.available() and device == 'cpu':
-        ref = ref_import.load()
-        net = ref.union.UNet3DModel('hr', **cfg).eval()
-        sd = R.seeded_state_dict({k: tuple(v.shape) for k, v in net.state_dict().items()}, 0)
-        net.load_state_dict(sd)
-        doc = ref.dual_octree.DualOctree(octree)
-        doc.post_processing_for_docnn()
-        x = torch.randn(doc.total_num, cc, generator=g)
-
-        def step():
-            eps = net(unet_type='hr', x=x, doctree=doc, timesteps=ts, unet_lr=net.unet_lr, label=label)
-            return R.ddim_eps_update(x, eps, ls, lsn)
-        return step, 'reference'
     sd = R.seeded_state_dict(_state_shapes(cfg, cfg_name), 0)
     dg = R.DualGraph(octree)
     lr_cfg, hr_cfg = R.split_cfg(cfg)
@@ -239,7 +258,7 @@ def cpu_baseline(cfg, cfg_name, batch_full, sample_batch=4, timed=2, budget_s=15
     """reference path on the host cores: B = sample_batch of the shapes, thread sweep {8,16,32,64,cores} with one
     timed forward each (after one warm-up at the first setting), then `timed` forwards at the best setting."""
     cores = os.cpu_count() or 1
-    step, kind = baseline_step_fn(cfg, cfg_name, sample_batch, 'cpu', True)
+    step, kind = baseline_step_fn(cfg, cfg_name, sample_batch, 'cpu')
     sweep = sorted({t for t in (8, 16, 32, 64, cores) if t <= cores}) or [cores]
     t_start = time.perf_counter()
     results = {}
@@ -249,8 +268,8 @@ def cpu_baseline(cfg, cfg_name, batch_full, sample_batch=4, timed=2, budget_s=15
         for th in sweep:
             torch.set_num_threads(th)
             t0 = time.perf_counter(); step(); results[th] = time.perf_counter() - t0
-            # stop when the budget is spent or more threads have clearly stopped helping (oversubscribed hosts get
-            # 10x slower at the full core count: 100 s for one B=4 step on the 128-core GPU box)
+            # stop when the budget is spent or more threads have clearly stopped helping (an oversubscribed host can get
+            # many times slower at its full core count)
             if (time.perf_counter() - t_start > budget_s and len(results) >= 2) or results[th] > 1.25 * min(results.values()):
                 break
         best = min(results, key=results.get)
@@ -264,13 +283,13 @@ def cpu_baseline(cfg, cfg_name, batch_full, sample_batch=4, timed=2, budget_s=15
             'sweep_s_per_step': {str(k): round(v, 3) for k, v in results.items()},
             'sample': '%s U-Net step (fp32, torch CPU) on B=%d of the %d shapes; thread sweep %s, best %d threads: %.2f s '
                       'per B=%d step (best of %d timed), scaled linearly to B=%d'
-                      % ('unmodified reference modules under the ocnn shim' if kind == 'reference' else 'oracle port of the reference',
+                      % ('oracle port of the reference',
                          sample_batch, batch_full, sweep, best, dt, sample_batch, timed + 1, batch_full)}
 
 
 def library_baseline(cfg, cfg_name, batch, dev, timed=3):
     """the reference op sequence through ATen / cuBLAS on this GPU (fp32, as the reference computes)"""
-    step, kind = baseline_step_fn(cfg, cfg_name, batch, str(dev), False)
+    step, kind = baseline_step_fn(cfg, cfg_name, batch, str(dev))
     with torch.no_grad():
         step(); step()
         torch.cuda.synchronize(dev)
@@ -287,7 +306,7 @@ def library_baseline(cfg, cfg_name, batch, dev, timed=3):
 
 
 def run_reference(args):
-    """`--impl reference`: the reference's own CPU implementation of the path, timed on the host cores."""
+    """`--impl reference`: the reference path on the host cores (its oracle port, see cpu_baseline)."""
     rank = int(os.environ.get('RANK', '0'))
     if rank != 0:
         return
@@ -317,7 +336,7 @@ def workload_config(args, nodes, per_gpu):
          'global_batch': args.batch * (args.gpus if args.weak else 1), 'batch_per_gpu': per_gpu,
          'code_channels': latent_channels(args),
          'parallelism': 'dp%d (batch shard, no collective in the step loop)' % args.gpus,
-         'l2': 'no flush: one step streams several GB of activations (>> 126 MB L2)'}
+         'l2': 'no flush: one step streams several GB of activations (>> 50 MB L2)'}
     if nodes:
         c['nodes_per_gpu'] = nodes
     return c
@@ -338,6 +357,7 @@ def run_ours(args):
         raise SystemExit('bench.py --impl ours needs a CUDA device: octfusion_b200 has no CPU path')
     torch.cuda.set_device(local)
     dev = torch.device('cuda', local)
+    torch.manual_seed(0)               # default-initialised weights: the same inputs from run to run (--dump-outputs)
     if world > 1:
         dist.init_process_group('nccl', device_id=dev)
     if args.workload == 'vae':
@@ -350,7 +370,7 @@ def run_ours(args):
     act = torch.bfloat16 if args.dtype == 'bf16' else torch.float32
     net = randomise_(graph_unet_union.UNet3DModel('hr', **cfg), 0).to(dev).eval()
     # the job's shapes: every rank generates the same `batch` shapes; strong scaling keeps a contiguous block of them
-    # (BASELINE.json configs[2]: "batch 32 sharded over 8xB200"), weak scaling keeps them all
+    # (BASELINE.json configs[2]: "batch 32 sharded over 8 GPUs"), weak scaling keeps them all
     l4, l5 = synth_splits(args.batch, seed=0)
     if args.weak or world == 1:
         per_gpu = args.batch
@@ -415,6 +435,8 @@ def run_ours(args):
         dist.all_reduce(ms, op=dist.ReduceOp.MAX)
     ms_total = float(ms.item())
     clk = clocks.stop(t0, t1) if rank == 0 else None
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, {'latent': st.x, 'eps': st.eps})
     # strong scaling: one step of the job = all ranks' shards done; weak: every rank does a full batch per step
     value = (world if args.weak else 1) * args.steps / (ms_total / 1000.0)
     kernels_per_step = int(st.kernels_per_step)
@@ -470,9 +492,9 @@ def run_ours(args):
         # burst figure unless the timed region is long enough (>= 2 s) for the power cap to set the clocks
         long_run = ms_total >= 2000.0
         key = 'bf16_tflops_sustained' if long_run else 'bf16_tflops'
-        peak_tf = float(peaks.get(key, 1400.0 if long_run else 1590.0))
+        peak_tf = float(peaks.get(key, H100_BF16_TFLOPS))
         peak_src = ('MEASURED_PEAKS.json %s (of measured)' % key) if peaks else \
-            ('%.0f TF/s (of fallback)' % peak_tf)
+            ('%.0f TF/s (H100 SXM data sheet, dense bf16, 700 W; not reached on a power-limited card)' % peak_tf)
         agg = {}
         reps = 3
         for rep in range(reps + 1):
@@ -496,21 +518,11 @@ def run_ours(args):
         tot_by = sum(a['bytes'] for a in agg.values())
         if tot_ms > 0:
             ach = tot_fl / (tot_ms * 1e-3) / 1e12
-            traffic, traffic_src = None, None
-            for cand in ('tc_traffic_r02.json', 'tc_traffic_r01.json'):   # DRAM bytes of the same launches (ncu capture)
-                try:
-                    tj = json.load(open(os.path.join(ROOT, 'profiles', cand)))
-                    traffic = tj['dram_bytes_per_step'] / tj['launches_per_step']
-                    traffic_src = 'profiles/' + cand
-                    break
-                except Exception:  # noqa: BLE001
-                    pass
             nl = sum(a['launches'] for a in agg.values()) / reps
             roofline = {'kernel': 'gather_gemm_tc_kernel (all launches of one step)', 'bound': 'tensor',
-                        'achieved': ach, 'peak': peak_tf, 'unit': 'TFLOP/s', 'frac': ach / peak_tf, 'traffic': traffic,
-                        'traffic_unit': 'DRAM bytes per launch (ncu dram__bytes_read+write, mean over the step; %s)' % traffic_src,
+                        'achieved': ach, 'peak': peak_tf, 'unit': 'TFLOP/s', 'frac': ach / peak_tf, 'traffic': None,
                         'launches_per_step': nl, 'algorithmic_bytes_per_launch': tot_by / reps / max(nl, 1),
-                        'peak_source': peak_src, 'frac_of_sustained': ach / float(peaks.get('bf16_tflops_sustained', 1400.0)),
+                        'peak_source': peak_src, 'frac_of_sustained': ach / float(peaks.get('bf16_tflops_sustained', H100_BF16_TFLOPS)),
                         'ms_per_step_in_kernel': tot_ms / reps,
                         'algorithmic_gflop_per_step': tot_fl / reps / 1e9, 'algorithmic_gb_per_step': tot_by / reps / 1e9}
             per_layer = []
@@ -576,10 +588,12 @@ def run_vae(args, dev, rank, world, real_stdout):
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     e0.record()
     for _ in range(args.steps):
-        case['step']()
+        out = case['step']()
     e1.record()
     torch.cuda.synchronize()
     launches = _lib.launch_count() - c0
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, vae_outputs(out))
     ms = torch.tensor([e0.elapsed_time(e1)], device=dev)
     if world > 1:
         dist.all_reduce(ms, op=dist.ReduceOp.MAX)
@@ -590,7 +604,7 @@ def run_vae(args, dev, rank, world, real_stdout):
             peaks = json.load(open(os.path.join(ROOT, 'MEASURED_PEAKS.json')))
         except Exception:  # noqa: BLE001
             pass
-        hbm = float(peaks.get('hbm_gbs', 6650.0))
+        hbm = float(peaks.get('hbm_gbs', H100_HBM_GBS))
         gbs = case['algorithmic_bytes'] / (per * 1e-3) / 1e9
         line = {'metric': METRICS['vae'], 'value': (world if args.weak else 1) * 1000.0 / per, 'unit': 'passes/s', 'n_gpus': world,
                 'steps': args.steps, 'warmup': args.warmup, 'ms_per_step': per, 'higher_is_better': True,
@@ -600,10 +614,28 @@ def run_vae(args, dev, rank, world, real_stdout):
                 'roofline': {'kernel': 'whole encode+decode pass', 'bound': 'hbm', 'achieved': gbs, 'peak': hbm,
                              'unit': 'GB/s', 'frac': gbs / hbm, 'traffic': None,
                              'algorithmic_bytes_per_pass': case['algorithmic_bytes'],
-                             'peak_source': 'MEASURED_PEAKS.json hbm_gbs (of measured)' if peaks else '6650 GB/s (of fallback)'}}
+                             'peak_source': 'MEASURED_PEAKS.json hbm_gbs (of measured)' if peaks else
+                             '%.0f GB/s (H100 SXM data sheet HBM3)' % hbm}}
         os.write(real_stdout, (json.dumps(line) + '\n').encode())
     if world > 1:
         dist.barrier(); dist.destroy_process_group()
+
+
+def vae_outputs(out):
+    """the tensors of GraphVAE.decode_code's result, named by key and depth"""
+    found = {}
+
+    def walk(name, v):
+        if torch.is_tensor(v) and v.is_floating_point():
+            found[name] = v
+        elif isinstance(v, dict):
+            for k, x in v.items():
+                walk('%s_%s' % (name, k) if name else str(k), x)
+        elif isinstance(v, (list, tuple)):
+            for k, x in enumerate(v):
+                walk('%s_%d' % (name, k) if name else str(k), x)
+    walk('', out)
+    return found
 
 
 def main():

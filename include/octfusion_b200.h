@@ -1,5 +1,5 @@
 /*
- * octfusion_b200 -- C ABI of the B200 (sm_100a) kernels behind the OctFusion denoising
+ * octfusion_b200 -- C ABI of the H100 (sm_90a) kernels behind the OctFusion denoising
  * U-Net hot path.
  *
  * The reference (octree-nn/octfusion) has NO native layer on this path: every operator below
@@ -44,20 +44,6 @@ unsigned long long of_launch_count(void); /* kernels launched by this library so
  * mirror has a different size must refuse to run (a stale .so would otherwise read garbage pointers) */
 int of_abi_sizeof_gemm_args(void);
 int of_abi_sizeof_octree_levels(void);
-/* diagnostics: per-role clock64 stamps of CTA `block` of the following of_gather_gemm_tc launches are written to
- * buf [8][cap_per_region] (uint64); buf = NULL switches tracing off (tools/trace_tc.py decodes the stamps) */
-int of_tc_trace_set(void* buf, int32_t cap_per_region, int32_t block);
-/* kernel-variant switches of of_gather_gemm_tc (experiments / tests; a value outside the set keeps the current one):
- * mt in {1, 2}: 128-row tiles per CTA for N <= 128; uni in {0, 1, 2}: 1 = weight tile inside the gather ring's stage, 2 = deeper separate weight ring;
- * cg in {1, 2}: 2 = CTA pairs (tcgen05 cta_group::2) for the 256-wide tiles; layout in {0, 1}: order of the warp
- * roles (scheduling priority follows the warp id).  Defaults: environment OCTFUSION_TC_MT / _UNI / _CG / _LAYOUT, else
- * 2 / 1 / 1 / 0.  Small M (fewer 128-row tiles than SMs) overrides the tile shape: the widest shape that still fills the
- * SMs (gemm_tc.cu, of_gather_gemm_tc). */
-int of_tc_config(int32_t mt, int32_t uni, int32_t cg, int32_t layout);
-/* how of_gather_gemm_tc fills the gathered operand tiles: 1 = TMA tile::gather4 (one instruction per 4 neighbour rows,
- * tensor maps built per launch; needs 128-byte aligned rows), 0 = 16-byte cp.async copies by 8 producer warps.  Any other
- * value keeps the current mode.  Default: environment OCTFUSION_TC_TMAG, else 0. */
-int of_tc_gather_mode(int32_t tma);
 
 /* ------------------------------------------------------------------------------------------
  * Tap-gather GEMM:   out[m, :] = sum_tap  mean_{j in nbr(m, tap)} [ A[j, :] | onehot(type_j) ] . W[tap]
@@ -92,7 +78,7 @@ typedef struct of_gemm_args {
   int32_t a_silu;                                /* fp32 path only: apply SiLU to A on load   */
   /* B: fp32 path  -> canonical fp32 [K, N] row-major, K = taps*(c0+c1+ntype), k = tap*(c0+c1+ntype)+c
    *    (exactly GraphConv.weights; other layouts go through of_repack_weight once)
-   *    tcgen05 path -> bf16 tile image produced by of_pack_weight_tc                         */
+   *    tensor-core path -> bf16 tile image produced by of_pack_weight_tc                         */
   const void* w;
   const float* bias;                             /* [N] or NULL                               */
   const float* row_add; int64_t ld_row_add; const int32_t* row_add_idx;
@@ -102,7 +88,7 @@ typedef struct of_gemm_args {
   int32_t out_f32;                               /* 1: write fp32 regardless of dtype         */
   int32_t M, N;
   int32_t dtype;                                 /* activation dtype of a0/a1/resid/out       */
-  /* tcgen05 path only: slots with several neighbours read their pre-averaged row.  There tap_tab uses
+  /* tensor-core path only: slots with several neighbours read their pre-averaged row.  There tap_tab uses
    * the ORDINAL encoding of of_graph_multi_index: v <= -2 -> row -(v+2) of a_multi (built per input tensor
    * by of_gather_mean_rows); multi_types[ord] = per-type neighbour counts, 8 bits per type -- only read when
    * nt_block is NULL, and only exact while a slot has < 256 neighbours of one type (two adaptive levels: <= 16;
@@ -111,13 +97,13 @@ typedef struct of_gemm_args {
   const uint64_t* multi_types;
   /* row counts of a0 / a1 (informational; may be 0)                                                          */
   int32_t rows_a0, rows_a1;
-  /* tcgen05 path with ntype > 0 (required there): the node-type K block as a precomputed bf16 [M, 64] tensor
+  /* tensor-core path with ntype > 0 (required there): the node-type K block as a precomputed bf16 [M, 64] tensor
    * (of_graph_type_block, record-encoded table)                                                              */
   const void* nt_block;
-  /* tcgen05 path: 1 = walk the row tiles from the last to the first.  Alternating the direction from one kernel to
-   * the next lets each kernel start on the rows its producer wrote last, which are still in the 126 MB L2.  */
+  /* tensor-core path: 1 = walk the row tiles from the last to the first.  Alternating the direction from one kernel to
+   * the next lets each kernel start on the rows its producer wrote last, which are still in the 50 MB L2.  */
   int32_t reverse;
-  /* tcgen05 path, optional: group-norm partial statistics of the OUTPUT, computed in the epilogue from the fp32
+  /* tensor-core path, optional: group-norm partial statistics of the OUTPUT, computed in the epilogue from the fp32
    * values before they are rounded to bf16 (the statistics pass of the following DualOctreeGroupNorm,
    * modules.py:291-326, then never reads the tensor).  Rows are cut into 32-row chunks; a chunk is split into
    * SEGMENTS at every change of sample id; stat_chunk_seg [ceil(M/32)+1] is the exclusive prefix sum of segments
@@ -137,13 +123,13 @@ typedef struct of_gemm_args {
 /* CUDA-core FFMA path: any shape, fp32-exact accumulation order-insensitive to 1e-6. */
 int of_gather_gemm_simt(const of_gemm_args* args, void* stream);
 
-/* tcgen05 / TMEM path (bf16 operands, fp32 accumulate). Requires dtype = OF_BF16,
+/* Tensor-core path (wgmma, bf16 operands, fp32 accumulate). Requires dtype = OF_BF16,
  * (c0 % 64 == 0), (c1 % 64 == 0), N % 16 == 0 and w packed by of_pack_weight_tc. */
 int of_gather_gemm_tc(const of_gemm_args* args, void* stream);
 /* Split-K variant for launches whose row tiles cannot fill the GPU (the dense 4^3 / 8^3 levels: M = 2048 at B = 32, with
  * K up to 13824): of_tc_splitk_plan returns the number S of K ranges this library would use for `args` (1 = do not
  * split).  With S > 1 the caller provides a workspace of S * M * N floats and calls of_gather_gemm_tc_splitk: pass 1
- * runs the same tcgen05 kernel over (output tile, K range) pairs writing fp32 partial sums, pass 2 adds the ranges in
+ * runs the same tensor-core kernel over (output tile, K range) pairs writing fp32 partial sums, pass 2 adds the ranges in
  * order (bit-reproducible) with bias / row_add / resid, stores `out` and computes the stat_out statistics.  Same
  * arguments and results as of_gather_gemm_tc up to fp32 summation order. */
 int of_tc_splitk_plan(const of_gemm_args* args);
@@ -170,7 +156,7 @@ int of_repack_weight(const float* src, int64_t s_tap, int64_t s_c, int64_t s_n,
  * Statistics are deterministic (no atomics): rows are cut into 32-row chunks, chunks into per-sample SEGMENTS
  * (see of_gemm_args.stat_out), and every segment owns one slot of a partial buffer.
  *   stats:    part [n_segments, C/gran, 2] fp32 = (sum x, sum x^2) per granule of `gran` (2 or 4) channels of each segment, one thread
- *             per (chunk, channel vector), rows added in order.  The tcgen05 GEMM writes the same buffer from its
+ *             per (chunk, channel vector), rows added in order.  The tensor-core GEMM writes the same buffer from its
  *             epilogue (stat_out), in which case this pass is skipped.
  *             Slot of segment s in `part`: seg_slot[s] -- the segments of a sample occupy CONSECUTIVE slots (sample-major,
  *             row order inside the sample).
@@ -282,14 +268,14 @@ int of_graph_fill(const of_octree_levels* oct, int32_t D, const int32_t* need_of
 /* Multi-neighbour slots (coarse leaf next to a subdivided cell: 4..16 finer neighbours, averaged by
  * scatter_mean, utils/scatter.py:42-66; up to 4^k for k adaptive levels).  of_graph_multi_flags marks them (flags[i] = tap_tab[i] <= -2);
  * after an exclusive scan of the flags, of_graph_multi_index writes the ordinal-encoded table used by the
- * tcgen05 path (v <= -2 -> -(ordinal+2)), multi_off[ord] = offset of the slot's record in tap_extra, and
+ * tensor-core path (v <= -2 -> -(ordinal+2)), multi_off[ord] = offset of the slot's record in tap_extra, and
  * multi_types[ord] = packed per-type neighbour counts (8 bits per node type).
  * of_gather_mean_rows: out[ord, :] = mean over the slot's neighbours of (a0|a1)[row, :]  (per input tensor). */
 int of_graph_multi_flags(const int32_t* tap_tab, int64_t slots, int32_t* flags, void* stream);
 int of_graph_multi_index(const int32_t* tap_tab, const int32_t* tap_extra, const uint8_t* node_type,
                          int64_t slots, const int32_t* flag_scan, int32_t* tap_tab_ord, int32_t* multi_off,
                          uint64_t* multi_types, void* stream);
-/* Node-type K block of the tcgen05 GEMM, a per-graph constant: out [rows, 64] bf16, column tap*ntype + type =
+/* Node-type K block of the tensor-core GEMM, a per-graph constant: out [rows, 64] bf16, column tap*ntype + type =
  * (#neighbours of that type in slot (row, tap)) / (#neighbours) = the scatter_mean of the one-hot columns that
  * GraphConv.forward appends to the features (models/networks/modules.py:199-202, 208-210); zero elsewhere.
  * tap_tab / tap_extra are the RECORD-encoded tables of of_graph_fill.  Requires taps*ntype <= 64, ntype <= 8. */

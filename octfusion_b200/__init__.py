@@ -1,4 +1,4 @@
-"""octfusion_b200 -- B200 (sm_100a) kernels behind the OctFusion denoising U-Net hot path.
+"""octfusion_b200 -- H100 (sm_90a) kernels behind the OctFusion denoising U-Net hot path.
 
 Importing this package loads liboctfusion_b200.so; it raises if the library is missing (there is no
 CPU or library fallback).  Public surface mirrors the reference (octree-nn/octfusion):

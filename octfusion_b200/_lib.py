@@ -1,7 +1,7 @@
 """ctypes binding of liboctfusion_b200.so (the C ABI declared in include/octfusion_b200.h).
 
 There is NO CPU fallback: if the library cannot be loaded every operator raises.  The library
-is built in-tree by `octfusion_b200.build` (nvcc, sm_100a); when the .so is missing and nvcc is
+is built in-tree by `octfusion_b200.build` (nvcc, sm_90a); when the .so is missing and nvcc is
 available it is built on first import, otherwise the import fails loudly.
 """
 from __future__ import annotations
@@ -60,9 +60,6 @@ _PROTOS = {
     'of_launch_count': (C.c_ulonglong, []),
     'of_abi_sizeof_gemm_args': (C.c_int, []),
     'of_abi_sizeof_octree_levels': (C.c_int, []),
-    'of_tc_trace_set': (C.c_int, [_vp, _i32, _i32]),
-    'of_tc_config': (C.c_int, [_i32, _i32, _i32, _i32]),
-    'of_tc_gather_mode': (C.c_int, [_i32]),
     'of_gather_gemm_simt': (C.c_int, [C.POINTER(GemmArgs), _vp]),
     'of_gather_gemm_tc': (C.c_int, [C.POINTER(GemmArgs), _vp]),
     'of_tc_splitk_plan': (C.c_int, [C.POINTER(GemmArgs)]),
@@ -109,7 +106,7 @@ class LibraryMissing(ImportError):
     pass
 
 
-ABI_VERSION = 4          # of_version() of the header this binding mirrors
+ABI_VERSION = 5          # of_version() of the header this binding mirrors
 
 
 def _load():

@@ -1,7 +1,7 @@
-"""Compile the CUDA sources in csrc/ for sm_100a into octfusion_b200/lib/liboctfusion_b200.so.
+"""Compile the CUDA sources in csrc/ for sm_90a into octfusion_b200/lib/liboctfusion_b200.so.
 
-Plain nvcc, in-tree output (the .so travels to the GPU box with the repo snapshot; a JIT cache
-would not).  Cross-compiles without a GPU.  Re-runs only when a source is newer than the .so.
+Plain nvcc, in-tree output next to the package, so that the built tree is importable as it stands (a read-only
+tree included).  Cross-compiles without a GPU.  Re-runs only when a source is newer than the .so.
 """
 from __future__ import annotations
 import os
@@ -13,7 +13,7 @@ CSRC = os.path.join(HERE, 'csrc')
 LIBDIR = os.path.join(HERE, 'lib')
 LIB = os.path.join(LIBDIR, 'liboctfusion_b200.so')
 SOURCES = ['runtime.cu', 'gemm_simt.cu', 'gemm_tc.cu', 'norm.cu', 'attention.cu', 'misc.cu', 'graph.cu', 'mpu.cu']
-NVCC_FLAGS = ['-gencode', 'arch=compute_100a,code=sm_100a', '-O3', '-lineinfo', '-std=c++17',
+NVCC_FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-O3', '-lineinfo', '-std=c++17',
               '-Xcompiler', '-fPIC', '--expt-relaxed-constexpr', '--extended-lambda']
 
 

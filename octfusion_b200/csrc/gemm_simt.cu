@@ -2,7 +2,7 @@
 //
 //   out[m,:] = sum_tap mean_{j in nbr(m,tap)} [A[j,:] | onehot(type_j)] . W[tap]  (+bias +row_add +resid)
 //
-// Replaces, for shapes the tcgen05 kernel does not take (fp32 activations, Cin = 3, Cout = 3,
+// Replaces, for shapes the tensor-core kernel does not take (fp32 activations, Cin = 3, Cout = 3,
 // the [B,512] embedding MLPs) the reference op sequence  x[col] -> scatter_mean -> view @ W
 // (reference models/networks/modules.py:194-220, diffusion_networks/utils/scatter.py:42-66),
 // nn.Linear / Conv1x1 (modules.py:332-339) and dense Conv3d (modules.py:493-502) in fp32 mode.
@@ -142,7 +142,7 @@ extern "C" int of_gather_gemm_simt(const of_gemm_args* args, void* stream) {
   int rc = of::check_gemm_args(args, "of_gather_gemm_simt");
   if (rc) return rc;
   if (args->stat_out != nullptr) {
-    of::set_error("of_gather_gemm_simt: stat_out is a tcgen05-path feature (run of_gn_stats on the output instead)");
+    of::set_error("of_gather_gemm_simt: stat_out is a tensor-core-path feature (run of_gn_stats on the output instead)");
     return OF_E_UNSUPPORTED;
   }
   if (args->M == 0) return OF_OK;

@@ -1,41 +1,33 @@
-// Tap-gather GEMM on the 5th-generation tensor cores (tcgen05.mma, accumulators in TMEM).
+// Tap-gather GEMM on the Hopper tensor cores (wgmma.mma_async, fp32 accumulators in registers).
 //
 //   out[m,:] = sum_tap mean_{j in nbr(m,tap)} [A[j,:] | onehot(type_j)] . W[tap]  (+bias +row_add +resid)
 //
-// This is the B200 replacement of the reference's GraphConv op sequence
+// This replaces the reference's GraphConv op sequence
 //   x[col] (aten::index) -> scatter_mean into a [7N, C] buffer -> view(N, 7C) @ W
 // (reference models/networks/modules.py:194-220, diffusion_networks/utils/scatter.py:42-66) and of
 // its dense Conv3d / Conv1x1 / Down/Upsample GEMMs (modules.py:332-339, 392-395, 440-443, 493-502).
-// The im2col buffer is never written to HBM: gather warps build each [128 x 64] bf16 A tile
-// directly in shared memory, in the 128-byte-swizzled K-major layout tcgen05.mma reads.
+// The im2col buffer is never written to HBM: producer warps build each [128 x 64] bf16 A tile
+// directly in shared memory, in the 128-byte-swizzled K-major layout wgmma reads.
 //
-// One persistent CTA per SM, 512 threads, warp-specialised (role -> warp id: tc_roles() below; the default layout is):
-//   warps 0-3   epilogue: tcgen05.ld of the fp32 accumulator, +bias/+emb[batch]/+residual, store; optionally the
-//               group-norm partial statistics of the tile (warp-shuffle reduction, one write per 32-row chunk --
-//               no atomics, bit-reproducible): the statistics pass of the following DualOctreeGroupNorm
-//               (modules.py:291-326) never reads the tensor again
-//   warp  4     MMA issuer (elect.sync lane issues): tcgen05.mma 128 x BN x 16, tcgen05.commit releases the
-//               shared-memory stages; it never waits on an mbarrier for operands -- warp 14 (scout) does, and publishes
-//               the count of ready stages in shared memory
-//   warp  5     weight loader: cp.async.bulk (TMA 1-D) of pre-swizzled [BN x 64] tiles
-//   warps 6-13  gather producers (4 groups x 2 warps, each group owns every 4th 16 KB sub-tile):
-//               tap table -> sixteen 16-byte cp.async (LDGSTS) per thread straight into the swizzled A stage,
-//               completion by cp.async.mbarrier.arrive.noinc; no registers, no waiting.  The producers' address
-//               arithmetic is kept to 4 instructions per copy (it shares issue slots with the MMA warp).
-//               Opt-in alternative (TG = 1): the TMA gathers the rows, cp.async.bulk.tensor tile::gather4 (measured slower).
-// A CTA tile is MT (1 or 2) row tiles of 128 rows x BN columns; with MT = 2 (BN <= 128) one streamed weight tile
-// feeds both row tiles.  Pipelines: shared-memory ring(s) with full/empty mbarriers between {producers, loader} and
-// the MMA warp; two sets of TMEM accumulators (full/empty mbarriers) between MMA and epilogue, so tile i+1 is computed
-// while tile i drains.
+// One persistent CTA per SM, 384 threads = three warpgroups:
+//   warpgroup 0    producers: each warp fills every PW-th stage of the shared-memory ring (PW = 4, or the ring depth
+//                  when it is shallower).  Tap table -> thirty-two 16-byte cp.async (LDGSTS) per lane straight into the
+//                  swizzled A stage, completion by cp.async.mbarrier.arrive.noinc; lane 0 also streams the stage's
+//                  pre-swizzled [BN x 64] weight tile with cp.async.bulk (1-D TMA) onto the same full barrier.  The
+//                  table entries of the warp's next stage are fetched before it waits for the current one to be freed.
+//   warpgroups 1-2 consumers, 64 rows of the 128-row tile each: wgmma 64 x BN x 16 from shared memory into register
+//                  accumulators, one stage in flight; then the epilogue: accumulators -> shared-memory staging (64
+//                  columns at a time) -> +bias/+emb[batch]/+residual, store; optionally the group-norm partial statistics
+//                  of the tile (warp-shuffle reduction, one write per 32-row chunk -- no atomics, bit-reproducible): the
+//                  statistics pass of the following DualOctreeGroupNorm (modules.py:291-326) never reads the tensor again.
+// While the consumers drain a tile the producers already fill the ring with the next tile's stages.
 //
 // K is consumed as 64-wide blocks ordered (channel block outer, tap inner): the 7 (or 27) taps
 // of one 64-channel slab touch the same few hundred source rows, which then sit in L2.
 // The one-hot node-type columns (modules.py:199-202) are one extra K block of per-slot type fractions, read
 // from a per-graph precomputed tensor (of_graph_type_block); slots with several finer neighbours read a
 // pre-averaged row (of_gather_mean_rows); the weights are re-laid once by of_pack_weight_tc.
-// Measurements behind each of these choices: profiles/tc_gather_experiments_r0*.md.
 #include "common.cuh"
-#include <cuda.h>              // CUtensorMap (the encoder is fetched through cudaGetDriverEntryPoint: no -lcuda)
 #include <stdlib.h>
 #include <string.h>
 #include <type_traits>
@@ -44,23 +36,11 @@ namespace of {
 
 constexpr int TC_BM = 128;
 constexpr int TC_BK = 64;                 // bf16 elements = 128 bytes = one swizzle row
-constexpr int TC_EPI_WARPS = 4;                   // (8 = two per TMEM lane quarter was measured: no faster -- the drain is paced by TMEM reads)
-constexpr int TC_PROD_WARPS = 8;
-// Warp roles.  The SM's warp schedulers prefer the HIGHEST warp id among the eligible warps of a sub-partition
-// (measured, B300_MICROARCH.md), so the order of the roles is a scheduling-priority choice; which order is best was
-// settled by measurement (profiles/tc_gather_experiments_r02.md), hence a run-time layout id (TcParams::layout):
-//   0: epilogue 0-3 | MMA 4 | loader 5 | producers 6-13 | scout 14            (producers on top)
-//   1: idle 0 | scout 1 | loader 2 | MMA 3 | producers 4-11 | epilogue 12-15   (epilogue on top, then producers)
-// (measured identical: profiles/tc_gather_experiments_r02.md)
-// An epilogue warp e works on TMEM lane quarter e % 4, which must equal warp_id % 4: both layouts respect it.
-struct TcRoles { int scout, prod0, loader, mma, epi0; };
-__device__ __forceinline__ TcRoles tc_roles(int layout) {
-  if (layout == 1) return TcRoles{1, 4, 2, 3, 12};
-  return TcRoles{14, 6, 5, 4, 0};
-}
-constexpr int TC_THREADS = 16 * 32;                                    // 512
+constexpr int TC_THREADS = 3 * 128;
 constexpr int TC_MAX_TAPS = 27;
-constexpr int TC_GROUPS = 4;                // producer groups of 2 warps
+constexpr int TC_SMEM_MAX = 227 * 1024;   // opt-in dynamic shared memory per block on H100
+// setmaxnreg only moves registers inside the allocation made at launch (384 threads x 168): 128 * 96 + 256 * 200 <= 384 * 168
+constexpr int TC_PROD_REGS = 96, TC_CONS_REGS = 200;
 
 // ------------------------------------------------------------------------------------------------
 // PTX wrappers
@@ -87,217 +67,27 @@ __device__ __forceinline__ bool mbar_try_wait(uint32_t bar, uint32_t parity) {
       : "memory");
   return ok != 0;
 }
-__device__ __forceinline__ void st_release_cta(uint32_t addr, uint32_t v) {
-  asm volatile("st.release.cta.shared::cta.u32 [%0], %1;" ::"r"(addr), "r"(v) : "memory");
-}
-__device__ __forceinline__ uint32_t ld_acquire_cta(uint32_t addr) {
-  uint32_t v;
-  asm volatile("ld.acquire.cta.shared::cta.u32 %0, [%1];" : "=r"(v) : "r"(addr) : "memory");
-  return v;
-}
-// the same with cluster-scope acquire (the arrivals come from the peer CTA)
-__device__ __forceinline__ bool mbar_test_wait_cluster(uint32_t bar, uint32_t parity) {
-  uint32_t ok;
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "mbarrier.test_wait.parity.acquire.cluster.shared::cta.b64 p, [%1], %2;\n\t"
-      "selp.u32 %0, 1, 0, p;\n\t}"
-      : "=r"(ok)
-      : "r"(bar), "r"(parity)
-      : "memory");
-  return ok != 0;
-}
-// non-blocking probe of a phase (true = the phase with this parity has completed)
-__device__ __forceinline__ bool mbar_test_wait(uint32_t bar, uint32_t parity) {
-  uint32_t ok;
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "mbarrier.test_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-      "selp.u32 %0, 1, 0, p;\n\t}"
-      : "=r"(ok)
-      : "r"(bar), "r"(parity)
-      : "memory");
-  return ok != 0;
-}
-// Bounded wait: a protocol bug becomes a trap (an error the host sees), never a hung GPU.
-// variant for the long waits of the epilogue warps: back off between polls so that the four idle warps do not
-// compete with the producers for issue slots
-__device__ __forceinline__ void mbar_wait_relaxed(uint32_t bar, uint32_t parity) {
-  if (mbar_try_wait(bar, parity)) return;
-  const long long t0 = clock64();
-  while (!mbar_try_wait(bar, parity)) {
-    __nanosleep(200);
-    if (clock64() - t0 > 4000000000ll) {
-      printf("octfusion_b200 gemm_tc: mbarrier timeout (block %d thread %d bar %u parity %u)\n", (int)blockIdx.x,
-             (int)threadIdx.x, bar, parity);
-      __trap();
-    }
-  }
-}
+// Bounded wait: a protocol bug becomes a trap (an error the host sees), never a hung GPU.  (No printf here: a function
+// call inside the consumers' MMA loop would make ptxas serialise the wgmma pipeline.)
 __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
   if (mbar_try_wait(bar, parity)) return;
   const long long t0 = clock64();
   while (!mbar_try_wait(bar, parity)) {
-    if (clock64() - t0 > 4000000000ll) {
-      printf("octfusion_b200 gemm_tc: mbarrier timeout (block %d thread %d bar %u parity %u)\n", (int)blockIdx.x,
-             (int)threadIdx.x, bar, parity);
-      __trap();
-    }
+    if (clock64() - t0 > 4000000000ll) __trap();
   }
 }
-// one lane of a fully converged warp (elect.sync): the uniform-datapath instructions (UTCHMMA, UTCBAR, UBLKCP)
-// are then issued from converged code instead of the ELECT/BRA.U.ANY retry loops the compiler emits for a
-// divergent `if (lane == 0)` region
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred;
-  asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(pred));
-  return pred != 0;
-}
-__device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+// register budget of a warpgroup (the producers give theirs to the accumulators of the consumers)
+template <int R> __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R> __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
 __device__ __forceinline__ void fence_mbar_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
+// the stage was written by cp.async (generic proxy) and is read by wgmma (async proxy)
+__device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
 __device__ __forceinline__ void bulk_g2s(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar) {
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst),
                "l"(src), "r"(bytes), "r"(bar)
                : "memory");
 }
-__device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
-  asm volatile("mbarrier.expect_tx.relaxed.cta.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void tmem_alloc(uint32_t result_slot, uint32_t cols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(result_slot), "r"(cols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t cols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(cols) : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-// D[tmem] (+)= A[smem desc] * B[smem desc], bf16 x bf16 -> fp32, M=128, N=BN, K=16
-__device__ __forceinline__ void umma_bf16(uint32_t d_tmem, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                          uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// same, descriptors given by their low words; high word = SBO 1024 B (>>4 = 64) | version 1 @46 | SWIZZLE_128B (2) @61
-constexpr uint32_t TC_DESC_HI = 64u | (1u << 14) | (2u << 29);
-__device__ __forceinline__ void umma_bf16_lo(uint32_t d_tmem, uint32_t a_lo, uint32_t b_lo, uint32_t idesc,
-                                             uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t.reg .b64 da, db;\n\t"
-      "mov.b64 da, {%1, %5};\n\t"
-      "mov.b64 db, {%2, %5};\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %3, p;\n\t}" ::"r"(d_tmem),
-      "r"(a_lo), "r"(b_lo), "r"(idesc), "r"(accumulate), "r"(TC_DESC_HI)
-      : "memory");
-}
-
-// ---- CTA-pair (cta_group::2) variants: two CTAs of a cluster compute one 256-row tile, each staging its own 128 rows of
-// A and HALF of the weight tile (profiles/tc_gather_experiments_r02.md) ----
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// shared::cluster address of the same shared-memory location in CTA `rank` of the cluster
-__device__ __forceinline__ uint32_t map_to_cta(uint32_t local_addr, uint32_t rank) {
-  uint32_t r;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(local_addr), "r"(rank));
-  return r;
-}
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_addr) {
-  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
-}
-__device__ __forceinline__ void st_release_cluster(uint32_t cluster_addr, uint32_t v) {
-  asm volatile("st.release.cluster.shared::cluster.u32 [%0], %1;" ::"r"(cluster_addr), "r"(v) : "memory");
-}
-__device__ __forceinline__ uint32_t ld_acquire_cluster(uint32_t addr) {
-  uint32_t v;
-  asm volatile("ld.acquire.cluster.shared::cta.u32 %0, [%1];" : "=r"(v) : "r"(addr) : "memory");
-  return v;
-}
-__device__ __forceinline__ void tmem_alloc2(uint32_t result_slot, uint32_t cols) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(result_slot), "r"(cols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc2(uint32_t taddr, uint32_t cols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(cols) : "memory");
-}
-// commit of the pair's MMAs: arrives on the barrier at this offset in BOTH CTAs
-__device__ __forceinline__ void umma_commit2(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(bar),
-               "h"((uint16_t)3)
-               : "memory");
-}
-// D[tmem of both CTAs] (+)= A (128 rows from each CTA) * B (BN/2 weight rows from each CTA): M = 256, N = BN, K = 16
-__device__ __forceinline__ void umma_bf16_lo2(uint32_t d_tmem, uint32_t a_lo, uint32_t b_lo, uint32_t idesc,
-                                              uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t.reg .b64 da, db;\n\t"
-      "mov.b64 da, {%1, %5};\n\t"
-      "mov.b64 db, {%2, %5};\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], da, db, %3, p;\n\t}" ::"r"(d_tmem),
-      "r"(a_lo), "r"(b_lo), "r"(idesc), "r"(accumulate), "r"(TC_DESC_HI)
-      : "memory");
-}
-// K-major, SWIZZLE_128B operand descriptor (cute::UMMA::SmemDescriptor): start>>4 in [0,14),
-// LBO>>4 in [16,30) (unused for swizzled K-major: 1), SBO>>4 in [32,46) = 1024 B between 8-row
-// groups, version 1 in [46,48), layout type SWIZZLE_128B = 2 in [61,64).
-__device__ __forceinline__ uint64_t make_desc_sw128(uint32_t saddr) {
-  uint64_t d = 0;
-  d |= (uint64_t)((saddr & 0x3FFFFu) >> 4);
-  d |= (uint64_t)1 << 16;
-  d |= (uint64_t)(1024 >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
-  return d;
-}
-// cute::UMMA::InstrDescriptor: c_format F32=1 @4, a_format BF16=1 @7, b_format BF16=1 @10,
-// a/b K-major (0) @15/@16, N>>3 @17, M>>4 @24.
-__host__ __device__ constexpr uint32_t make_idesc_pair(int bn) {          // cta_group::2: M = 256
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(bn >> 3) << 17) | ((uint32_t)(256 >> 4) << 24);
-}
-__host__ __device__ constexpr uint32_t make_idesc(int bn) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(bn >> 3) << 17) | ((uint32_t)(TC_BM >> 4) << 24);
-}
-
-#define OF_TMEM_LD32(taddr, r)                                                                               \
-  asm volatile(                                                                                              \
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "                                                              \
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,"  \
-      "%27,%28,%29,%30,%31}, [%32];"                                                                         \
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),     \
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), \
-        "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]),          \
-        "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]),          \
-        "=r"(r[30]), "=r"(r[31])                                                                             \
-      : "r"(taddr)                                                                                           \
-      : "memory")
-#define OF_TMEM_LD16(taddr, r)                                                                               \
-  asm volatile(                                                                                              \
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "                                                              \
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"                                      \
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),     \
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]) \
-      : "r"(taddr)                                                                                           \
-      : "memory")
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
 __device__ __forceinline__ void named_bar_sync(int id, int threads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
 }
@@ -306,83 +96,101 @@ __device__ __forceinline__ uint4 ldg_nc_v4(const void* p) {
   asm volatile("ld.global.nc.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(r.x), "=r"(r.y), "=r"(r.z), "=r"(r.w) : "l"(p));
   return r;
 }
-__device__ __forceinline__ void sts_v4(uint32_t addr, const uint4& v) {
-  asm volatile("st.shared.v4.u32 [%0], {%1,%2,%3,%4};" ::"r"(addr), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
-}
 // 16-byte asynchronous global->shared copy (LDGSTS); src_bytes = 0 zero-fills the destination
 __device__ __forceinline__ void cp_async_16(uint32_t dst, const void* src, uint32_t src_bytes) {
   asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "r"(src_bytes) : "memory");
 }
-// the same through L1 (experiment: neighbouring taps of one tile gather overlapping row sets)
-__device__ __forceinline__ void cp_async_16_ca(uint32_t dst, const void* src, uint32_t src_bytes) {
-  asm volatile("cp.async.ca.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "r"(src_bytes) : "memory");
-}
 __device__ __forceinline__ void cp_async_mbar_arrive_noinc(uint32_t bar) {
   asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(bar) : "memory");
 }
-__device__ __forceinline__ void cp_async_mbar_arrive(uint32_t bar) {
-  asm volatile("cp.async.mbarrier.arrive.shared::cta.b64 [%0];" ::"r"(bar) : "memory");
-}
-// TMA gather (Blackwell tile::gather4): four rows of a 2-D tensor, chosen by four row coordinates, land as four
-// consecutive 128-byte rows of a 128B-swizzled shared-memory tile; a coordinate outside the tensor reads as zeros.
-__device__ __forceinline__ void tma_gather4(uint32_t dst, const void* map, int col, int r0, int r1, int r2, int r3,
-                                            uint32_t bar) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.tile::gather4.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4, %5, %6}], [%7];"
-      ::"r"(dst), "l"(map), "r"(col), "r"(r0), "r"(r1), "r"(r2), "r"(r3), "r"(bar)
-      : "memory");
-}
-// one row (box 64 x 1) through the same kind of tensor map
-__device__ __forceinline__ void tma_row(uint32_t dst, const void* map, int col, int row, uint32_t bar) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];"
-      ::"r"(dst), "l"(map), "r"(col), "r"(row), "r"(bar)
-      : "memory");
-}
-__device__ __forceinline__ void sts_u16(uint32_t addr, uint16_t v) {
-  asm volatile("st.shared.u16 [%0], %1;" ::"r"(addr), "h"(v) : "memory");
-}
 
+// K-major, SWIZZLE_128B wgmma operand descriptor: start>>4 in [0,14), LBO>>4 in [16,30) (unused for swizzled K-major: 1),
+// SBO>>4 in [32,46) = 1024 B between 8-row groups, layout type SWIZZLE_128B = 1 in [62,64).  One 16-element K step is
+// +32 bytes = +2 in the start field (the tile bases are 1024-byte aligned).
+__device__ __forceinline__ uint64_t make_desc_sw128(uint32_t saddr) {
+  uint64_t d = 0;
+  d |= (uint64_t)((saddr & 0x3FFFFu) >> 4);
+  d |= (uint64_t)1 << 16;
+  d |= (uint64_t)(1024 >> 4) << 32;
+  d |= (uint64_t)1 << 62;
+  return d;
+}
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accumulator reads / writes across the asynchronous MMAs
+__device__ __forceinline__ void fence_operand(float& r) { asm volatile("" : "+f"(r)::"memory"); }
 
+// D[64 x N] (+)= A[64 x 16] * B[16 x N], both operands K-major in shared memory, bf16 x bf16 -> fp32.  Accumulator
+// fragment of thread t of the warpgroup: d[i] holds row 16*(t/32) + (t%32)/4 + 8*((i/2)%2), column 8*(i/4) + 2*(t%4) + i%2.
+template <int N> struct Wgmma;
+template <> struct Wgmma<16> {
+  static __device__ __forceinline__ void mma(float* d, uint64_t da, uint64_t db, uint32_t acc) {
+    asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %10, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1, 0, 0;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+      : "l"(da), "l"(db), "r"(acc));
+  }
+};
+template <> struct Wgmma<32> {
+  static __device__ __forceinline__ void mma(float* d, uint64_t da, uint64_t db, uint32_t acc) {
+    asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %18, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, 0, 0;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "l"(da), "l"(db), "r"(acc));
+  }
+};
+template <> struct Wgmma<64> {
+  static __device__ __forceinline__ void mma(float* d, uint64_t da, uint64_t db, uint32_t acc) {
+    asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %34, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(da), "l"(db), "r"(acc));
+  }
+};
+template <> struct Wgmma<128> {
+  static __device__ __forceinline__ void mma(float* d, uint64_t da, uint64_t db, uint32_t acc) {
+    asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %66, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(da), "l"(db), "r"(acc));
+  }
+};
+template <> struct Wgmma<256> {
+  static __device__ __forceinline__ void mma(float* d, uint64_t da, uint64_t db, uint32_t acc) {
+    asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %130, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n256k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, %96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, %112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, %128, %129, p, 1, 1, 0, 0;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]), "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]), "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]), "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]), "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]), "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]), "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+      : "l"(da), "l"(db), "r"(acc));
+  }
+};
 // ------------------------------------------------------------------------------------------------
 // shared-memory plan
 // ------------------------------------------------------------------------------------------------
-// BN  : output columns per tile (UMMA N)
-// MT  : 128-row sub-tiles per CTA tile (1 or 2).  With MT = 2 one streamed weight tile feeds two row tiles (two TMEM
-//       accumulators), which halves the weight bytes per SM (L2 -> shared memory -> tensor core) and the number of
-//       pipeline hand-shakes per MMA for the narrow (BN <= 128) layers.
-// UNI : 1 = the weight tile lives in the same ring stage as the gathered tiles (one full / one empty barrier per stage:
-//       the MMA warp waits once and commits once per stage); 0 = two independent rings (deeper gather ring).
-// CG  : 2 = CTA pair (cta_group::2): the pair computes a 256-row x BN tile; each CTA gathers its own 128 rows and streams
-//       only HALF of the weight tile, the tensor cores of both SMs read both halves -- half the weight bytes through
-//       each SM's shared memory, one MMA-issuing warp for two SMs.
-template <int BN, int MT, int UNI, int CG = 1>
+// BN: output columns per tile (the wgmma N).  A stage holds one 64-wide K block of the 128-row A tile and of the weight
+// tile; the ring takes what is left of the 227 KB beside the epilogue staging and the barriers.
+template <int BN>
 struct TcCfg {
-  // K blocks per stage.  The MMA warp spends ~0.25 us of waits, election, descriptor set-up and commits per stage; a
-  // stage must therefore hold >= 8 MMAs of a narrow tile (profiles/tc_gather_experiments_r01.md): either two K blocks
-  // of one row tile (MT = 1) or one K block of two row tiles (MT = 2).
-  static constexpr int KSUB = (MT == 1 && BN <= 128) ? 2 : 1;
-  static constexpr int SUBS = KSUB * MT;                            // 16 KB gathered sub-tiles per stage
-  static constexpr int A_SUB_BYTES = TC_BM * 128;                   // one K block of one row tile
-  static constexpr int B_SUB_BYTES = (BN / CG) * 128;               // one K block of B (a CTA pair stages half each)
-  static constexpr int A_BYTES = SUBS * A_SUB_BYTES;
-  static constexpr int B_BYTES = KSUB * B_SUB_BYTES;
-  static constexpr int BUDGET = 212 * 1024;
-  static constexpr bool UNIFIED = UNI == 1;
-  static constexpr int STAGE_BYTES = UNIFIED ? A_BYTES + B_BYTES : A_BYTES;
-  // depth of the weight ring.  Its round trip (commit -> MMAs retire -> slot free -> loader wakes -> bulk copy from L2
-  // lands -> scout -> MMA warp) is ~2500 cycles, ~3500 for a pair (two more hops): the ring must hold round trip / stage
-  // time slots or it paces the whole pipeline (profiles/tc_gather_experiments_r02.md)
-  static constexpr int B_STAGES = UNIFIED ? 0 : CG == 2 ? (UNI == 2 ? 8 : 6) : (KSUB > 1) ? 2 : (UNI == 2 ? 4 : 3);
-  static constexpr int A_STAGES = (BUDGET - B_STAGES * B_BYTES) / STAGE_BYTES;
-  static constexpr int ACC_COLS = 2 * MT * BN;                      // two accumulator sets (MMA of tile i+1 || epilogue of tile i)
-  static constexpr int TMEM_COLS = ACC_COLS <= 32 ? 32 : ACC_COLS <= 64 ? 64 : ACC_COLS <= 128 ? 128 : ACC_COLS <= 256 ? 256 : 512;
-  static constexpr int AUX_BYTES = 1024 + TC_EPI_WARPS * 1024;      // mbarriers, tmem slot, ready flags | per-epilogue-warp row of (bias + emb)
-  static constexpr int RING_BYTES = A_STAGES * STAGE_BYTES + B_STAGES * B_BYTES;
-  static constexpr int SMEM_BYTES = 1024 /*align slack*/ + RING_BYTES + AUX_BYTES;
-  static_assert(A_STAGES >= 2 && A_STAGES <= 16 && B_STAGES <= 8, "ring depth");
-  static_assert(ACC_COLS <= 512, "TMEM");
-  static_assert(CG == 1 || (MT == 1 && KSUB == 1), "the pair variant is built for the wide tiles");
+  static constexpr int A_BYTES = TC_BM * 128;
+  static constexpr int B_BYTES = BN * 128;
+  static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
+  static constexpr int EPI_COLS = BN < 64 ? BN : 64;                // columns per epilogue round
+  static constexpr int EPI_LD = EPI_COLS + 4;                       // staging row stride in floats (conflict-free float4 rows)
+  static constexpr int EPI_BYTES = 2 * 64 * EPI_LD * 4;             // one 64-row block per consumer warpgroup
+  static constexpr int AUX_BYTES = 1024 + 8 * 1024;                 // mbarriers | per-consumer-warp row of (bias + emb)
+  static constexpr int FIT = (TC_SMEM_MAX - 1024 - EPI_BYTES - AUX_BYTES) / STAGE_BYTES;
+  static constexpr int STAGES = FIT > 16 ? 16 : FIT;
+  // producer warps.  A warp that waits for the release of its slot must know that the slot's previous use has been
+  // released as well (the mbarrier parity tells two phases apart, not three): PW <= STAGES guarantees it.
+  static constexpr int PW = STAGES < 4 ? STAGES : 4;
+  static constexpr int SMEM_BYTES = 1024 /*align slack*/ + STAGES * STAGE_BYTES + EPI_BYTES + AUX_BYTES;
+  static_assert(STAGES >= 2 && SMEM_BYTES <= TC_SMEM_MAX, "ring depth");
 };
 
 struct TcParams {
@@ -392,22 +200,8 @@ struct TcParams {
                      // writing fp32 partial sums to its own [M, N] slab of the workspace (of_gather_gemm_tc_splitk)
   int cblocks;       // (c0+c1)/64
   int npad;          // N rounded up to 16 (rows per K block in the packed weight image)
-  int m_tiles, n_tiles;   // m_tiles counts CTA tiles of 128*MT rows
-  int layout;        // warp-role layout id (tc_roles)
-  int debug;         // OCTFUSION_TC_DEBUG bit mask (timing experiments only): 1 no gather, 2 no weight copy, 4 no epilogue I/O, 8 no MMA, 32 no tap-table reads, 64 gather through L1 (cp.async.ca)
-  unsigned long long* trace;   // of_tc_trace_set: per-role clock64 stamps of one CTA (diagnostics), or NULL
-  int trace_cap, trace_block;
-  // TG = 1: tensor maps (bf16, box 64 x 1, 128B swizzle) of a0, a1, the mean rows and the node-type block
-  CUtensorMap tm_a0, tm_a1, tm_multi, tm_nt;
+  int m_tiles, n_tiles;
 };
-
-// trace regions (each trace_cap stamps): 0 MMA warp (4 per stage: loop top, stage ready, MMAs issued, committed), 1 weight loader (2 per stage:
-// slot free, issued), 2..5 producer groups (3 per slot: loop top, slot free, issued), 6 epilogue warp 0 (2 per tile),
-// 7 scout (1 per stage, indexed by stage: the moment it saw the stage's full barrier complete)
-__device__ __forceinline__ void trace_put(const TcParams& p, int region, int& n, bool on) {
-  if (on && n < p.trace_cap) p.trace[(size_t)region * p.trace_cap + n] = (unsigned long long)clock64();
-  ++n;
-}
 
 // Sum of a[0..NV-1] (NV = 16 or 32) over the 32 lanes of the warp by recursive halving: NV = 16: 8+4+2+1+1 = 16 shuffles,
 // afterwards a[0] of lane L holds the warp total of the ORIGINAL a[(L >> 1) & 15]; NV = 32: 16+8+4+2+1 = 31 shuffles,
@@ -431,231 +225,298 @@ __device__ __forceinline__ void warp_reduce_vals(float (&a)[NV], int lane) {
 // ------------------------------------------------------------------------------------------------
 // the kernel
 // ------------------------------------------------------------------------------------------------
-// TG = 1: the gathered tiles are filled by the TMA (tile::gather4, one instruction per 4 rows, one warp per 16 KB
-// sub-tile) instead of 16-byte cp.async copies of 8 producer warps.
-// SK = 1: split-K instantiation (TcParams::ksplit K ranges per output tile).  A template parameter, not a run-time test: the
-// tile-index arithmetic and the extra live values of the split path cost registers in the epilogue (measured: +10 % on the
-// epilogue-bound layers when every launch carried them), so the common SK = 0 kernels are compiled without.
-template <int BN, int MT, int UNI, int CG, int TG, int SK>
+template <int BN>
 __global__ void __launch_bounds__(TC_THREADS, 1) gather_gemm_tc_kernel(const __grid_constant__ TcParams p) {
-  const int ksplit = SK ? p.ksplit : 1;                    // (compile-time 1 for SK = 0: the divisions below fold away)
-  using Cfg = TcCfg<BN, MT, UNI, CG>;
-  constexpr bool U1 = Cfg::UNIFIED;                        // weight tile inside the gather ring's stage
-  constexpr int KSUB = Cfg::KSUB, SUBS = Cfg::SUBS;
+  using Cfg = TcCfg<BN>;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  uint8_t* smem_gen = smem_raw + (smem_base - smem_u32(smem_raw));
-  const uint32_t stage_base = smem_base;
-  const uint32_t b_ring = smem_base + Cfg::A_STAGES * Cfg::STAGE_BYTES;      // (UNI = 0 only)
-  const uint32_t aux = smem_base + Cfg::RING_BYTES;
-  // aux layout: full[16] | empty[16] | b_full[8] | b_empty[8] | tmem_full[2] | tmem_empty[2] | tmem slot | flags | peer barriers
-  const uint32_t bar_full = aux, bar_empty = aux + 128;
-  const uint32_t bar_bfull = aux + 256, bar_bempty = aux + 320;
-  const uint32_t bar_tfull = aux + 384, bar_tempty = aux + 400;
-  const uint32_t tmem_slot = aux + 416;
-  // per ring slot: number of completed fills, published by the scout warp (A slots: 16 words, B slots: 8 words)
-  const uint32_t flag_a = aux + 448, flag_b = aux + 512;
-  // CG = 2, leader: "the peer's stage is full" barriers, one per ring slot (the peer's scout arrives remotely)
-  const uint32_t bar_pfull = aux + 576, bar_pbfull = aux + 704;
-  volatile uint32_t* tmem_slot_gen = reinterpret_cast<volatile uint32_t*>(smem_gen + Cfg::RING_BYTES + 416);
+  const uint32_t epi = smem_base + Cfg::STAGES * Cfg::STAGE_BYTES;
+  const uint32_t aux = epi + Cfg::EPI_BYTES;
+  const uint32_t bar_full = aux, bar_empty = aux + 128;             // one pair per ring slot
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const TcRoles W = tc_roles(p.layout);
+  const int wg = threadIdx.x >> 7, t = threadIdx.x & 127;
+  const int warp = t >> 5, lane = t & 31;
   const of_gemm_args& g = p.g;
   const int taps = g.taps;
-  // work items: CTA tiles of 128*MT rows (CG = 1) or pair tiles of 256 rows that both CTAs of a pair walk together
+  const int ksplit = p.ksplit;
   const int total_tiles = p.m_tiles * p.n_tiles * ksplit;   // virtual tile v: output tile v / ksplit, K range v % ksplit
-  uint32_t rank = 0;
-  if constexpr (CG == 2) rank = cluster_ctarank();
-  const int w_first = CG == 2 ? (int)(blockIdx.x >> 1) : (int)blockIdx.x;
-  const int w_stride = CG == 2 ? (int)(gridDim.x >> 1) : (int)gridDim.x;
-  constexpr int TILE_ROWS = TC_BM * MT * CG;
-  const bool tr = p.trace != nullptr && (int)blockIdx.x == p.trace_block;
 
-  if (warp == W.mma && lane == 0) {
-    for (int s = 0; s < Cfg::A_STAGES; ++s) {
-      // every producer thread of the stage's sub-tiles (TMA gather: one expect_tx arrival per warp = half sub-tile)
-      // (+ the weight loader's expect_tx arrival when the ring is shared)
-      mbar_init(bar_full + 8 * s, (TG ? 2 * SUBS : SUBS * (TC_PROD_WARPS / TC_GROUPS) * 32) + (U1 ? 1 : 0));
-      mbar_init(bar_empty + 8 * s, 1);
-    }
-    for (int s = 0; s < Cfg::B_STAGES; ++s) {
-      mbar_init(bar_bfull + 8 * s, 1);
-      mbar_init(bar_bempty + 8 * s, 1);
-    }
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(bar_tfull + 8 * a, 1);
-      mbar_init(bar_tempty + 8 * a, CG * TC_EPI_WARPS * 32);      // CG = 2: the epilogues of both CTAs
-    }
-    for (int i = 0; i < 24; ++i) st_release_cta(flag_a + 4 * i, 0u);
-    if constexpr (CG == 2) {
-      for (int s = 0; s < Cfg::A_STAGES; ++s) mbar_init(bar_pfull + 8 * s, 1);
-      for (int s = 0; s < Cfg::B_STAGES; ++s) mbar_init(bar_pbfull + 8 * s, 1);
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < Cfg::STAGES; ++s) {
+      mbar_init(bar_full + 8 * s, 32 + 1);                  // the producer warp's lanes + the weight copy's expect_tx
+      mbar_init(bar_empty + 8 * s, 2);                      // the two consumer warpgroups
     }
     fence_mbar_init();
   }
-  if (warp == W.mma) {                                     // CG = 2: the same warp of BOTH CTAs issues the paired alloc
-    if constexpr (CG == 2) tmem_alloc2(tmem_slot, Cfg::TMEM_COLS);
-    else tmem_alloc(tmem_slot, Cfg::TMEM_COLS);
-  }
-  tc_fence_before();
   __syncthreads();
-  if constexpr (CG == 2) cluster_sync_all();               // barriers / flags of both CTAs exist before any remote access
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot_gen;
 
-  if (warp >= W.epi0 && warp < W.epi0 + TC_EPI_WARPS) {
-    // =========================== epilogue ===========================
-    const int ew = warp - W.epi0;                        // 0..TC_EPI_WARPS-1
-    const int qw = ew & 3, chalf = ew >> 2;              // TMEM lane quarter (= warp id % 4) | which column chunks
-    const int r = qw * 32 + lane;
-    int it = 0, tn = 0;
-    for (int tile = w_first; tile < total_tiles; tile += w_stride, ++it) {
+  if (wg == 0) {
+    // =========================== producers ===========================
+    setmaxnreg_dec<TC_PROD_REGS>();
+    if (warp < Cfg::PW) {
+      const int q = lane & 7;                              // 16-byte chunk of the 128-byte row
+      const int rbase = lane >> 3;                         // rows rbase + 4 i
+      const __nv_bfloat16* a0 = reinterpret_cast<const __nv_bfloat16*>(g.a0);
+      const __nv_bfloat16* a1 = reinterpret_cast<const __nv_bfloat16*>(g.a1);
+      const int32_t* __restrict__ tab = g.tap_tab;
+      const uint8_t* wp = reinterpret_cast<const uint8_t*>(g.w);
+      const int my_tiles = (total_tiles - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;
+      const int total_stages = my_tiles * p.num_kb;
+      struct Pos { int m0, n0, kabs; };
+      // stage s of this CTA -> rows, columns and ABSOLUTE K block (split-K: the K range's offset included)
+      auto pos_of = [&](int s) {
+        const int ti = s / p.num_kb, kb = s - ti * p.num_kb;
+        const int tile = (int)blockIdx.x + ti * (int)gridDim.x;
+        const int vtile = g.reverse ? total_tiles - 1 - tile : tile;
+        const int ptile = vtile / ksplit;
+        return Pos{(ptile / p.n_tiles) * TC_BM, (ptile % p.n_tiles) * BN, (vtile - ptile * ksplit) * p.num_kb + kb};
+      };
+      auto fetch_taps = [&](const Pos& c, int32_t (&tv)[32]) {
+        const int cb = c.kabs / taps;
+        if (cb >= p.cblocks) return;                        // the node-type block
+        const int tap = c.kabs - cb * taps;
+#pragma unroll
+        for (int i = 0; i < 32; ++i) {
+          const int m = c.m0 + rbase + 4 * i;
+          tv[i] = -1;
+          if (m < g.M)
+            tv[i] = tab != nullptr ? __ldg(tab + ((uint32_t)m * (uint32_t)taps + (uint32_t)tap))   // < 2^31 (checked on host)
+                                   : (g.in_rows != nullptr ? __ldg(g.in_rows + m) : m);
+        }
+      };
+      int32_t tnext[32];
+#pragma unroll
+      for (int i = 0; i < 32; ++i) tnext[i] = -1;
+      if (warp < total_stages) fetch_taps(pos_of(warp), tnext);
+      for (int s = warp; s < total_stages; s += Cfg::PW) {
+        const Pos c = pos_of(s);
+        int32_t tv[32];
+#pragma unroll
+        for (int i = 0; i < 32; ++i) tv[i] = tnext[i];
+        if (s + Cfg::PW < total_stages) fetch_taps(pos_of(s + Cfg::PW), tnext);
+        const int stage = s % Cfg::STAGES;
+        const uint32_t phase = (uint32_t)(s / Cfg::STAGES) & 1u;
+        mbar_wait(bar_empty + 8 * stage, phase ^ 1);
+        const uint32_t a_addr = smem_base + stage * Cfg::STAGE_BYTES;
+        const uint32_t full = bar_full + 8 * stage;
+        if (lane == 0) {
+          mbar_arrive_expect_tx(full, (uint32_t)Cfg::B_BYTES);
+          bulk_g2s(a_addr + Cfg::A_BYTES, wp + ((int64_t)c.kabs * p.npad + c.n0) * 128, Cfg::B_BYTES, full);
+        }
+        const int cb = c.kabs / taps;
+        if (cb < p.cblocks) {
+          const int ch = cb * TC_BK;
+          const __nv_bfloat16* src;
+          int64_t ld;
+          if (ch < g.c0) { src = a0 + ch; ld = g.lda0; } else { src = a1 + (ch - g.c0); ld = g.lda1; }
+          src += q * 8;
+          const __nv_bfloat16* msrc = reinterpret_cast<const __nv_bfloat16*>(g.a_multi) + ch + q * 8;
+          // one neighbour -> its row; none -> zero fill; several -> the pre-averaged row of a_multi
+          const uint64_t sbase = reinterpret_cast<uint64_t>(src), mbase = reinterpret_cast<uint64_t>(msrc);
+          const uint32_t ldb = (uint32_t)ld * 2u, ldmb = (uint32_t)g.ld_multi * 2u;   // row strides in bytes
+          int32_t lo = tv[0];
+#pragma unroll
+          for (int i = 1; i < 32; ++i) lo = min(lo, tv[i]);
+          if (!__any_sync(0xffffffffu, lo < -1)) {
+#pragma unroll
+            for (int i = 0; i < 32; ++i) {
+              const int row = rbase + 4 * i;
+              const int32_t v = tv[i];
+              const uint64_t addr = sbase + (uint64_t)(uint32_t)max(v, 0) * (uint64_t)ldb;
+              cp_async_16(a_addr + row * 128 + ((q ^ (row & 7)) << 4), reinterpret_cast<const void*>(addr), v == -1 ? 0u : 16u);
+            }
+          } else {
+#pragma unroll
+            for (int i = 0; i < 32; ++i) {
+              const int row = rbase + 4 * i;
+              const int32_t v = tv[i];
+              const bool multi = v < -1;
+              const uint32_t idx = multi ? (uint32_t)(-2 - v) : (uint32_t)(v < 0 ? 0 : v);
+              const uint64_t addr = (multi ? mbase : sbase) + (uint64_t)idx * (uint64_t)(multi ? ldmb : ldb);
+              cp_async_16(a_addr + row * 128 + ((q ^ (row & 7)) << 4), reinterpret_cast<const void*>(addr), v == -1 ? 0u : 16u);
+            }
+          }
+        } else {
+          // node-type block, precomputed per graph (of_graph_type_block): a plain coalesced copy of rows m0..m0+127
+          const __nv_bfloat16* nb = reinterpret_cast<const __nv_bfloat16*>(g.nt_block) + q * 8;
+#pragma unroll
+          for (int i = 0; i < 32; ++i) {
+            const int row = rbase + 4 * i;
+            const int m = c.m0 + row;
+            cp_async_16(a_addr + row * 128 + ((q ^ (row & 7)) << 4), m < g.M ? (const void*)(nb + (int64_t)m * 64) : (const void*)nb,
+                        m < g.M ? 16u : 0u);
+          }
+        }
+        // one counted arrival per lane: it fires when this lane's cp.asyncs have landed
+        cp_async_mbar_arrive_noinc(full);
+      }
+    }
+  } else {
+    // =========================== consumers: MMA + epilogue ===========================
+    setmaxnreg_inc<TC_CONS_REGS>();
+    const int cw = wg - 1;                                 // rows 64 cw .. 64 cw + 63 of the tile
+    float acc[BN / 2];
+    int stage = 0;
+    uint32_t phase = 0;
+    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
       const int vtile = g.reverse ? total_tiles - 1 - tile : tile;
       const int ptile = vtile / ksplit;
       const int64_t split_row0 = (int64_t)(vtile - ptile * ksplit) * g.M;        // this K range's slab of the workspace
-      const int mt0 = (ptile / p.n_tiles) * TILE_ROWS + (int)rank * TC_BM, n0 = (ptile % p.n_tiles) * BN;
-      const int as = it & 1;
-      mbar_wait_relaxed(bar_tfull + 8 * as, (it >> 1) & 1);
-      tc_fence_after();
-      if (ew == 0 && lane == 0) trace_put(p, 6, tn, tr);
-#pragma unroll 1
-      for (int h = 0; h < MT; ++h) {
-        const int m = mt0 + h * TC_BM + r;
-        const bool row_ok = m < g.M;
-        const int64_t orow = row_ok ? (g.out_rows ? (int64_t)g.out_rows[m] : (int64_t)m + split_row0) : 0;
-        const float* radd = (row_ok && g.row_add) ? g.row_add + (int64_t)g.row_add_idx[m] * g.ld_row_add : nullptr;
-        const __nv_bfloat16* res =
-            (row_ok && g.resid) ? reinterpret_cast<const __nv_bfloat16*>(g.resid) + (int64_t)m * g.ld_resid : nullptr;
-        // ---- group-norm partial statistics of this 32-row chunk (see of_gemm_args.stat_out); set up first so that its
-        // index loads are in flight together with those of the staging below ----
-        int seg0 = 0, nseg = 0, my_seg = 0, my_slot = 0;
-        if (g.stat_out != nullptr) {
-          const int chunk = (mt0 + h * TC_BM) / 32 + qw;
-          if (chunk * 32 < g.M) {
-            seg0 = __ldg(g.stat_chunk_seg + chunk);
-            nseg = __ldg(g.stat_chunk_seg + chunk + 1) - seg0;
-            if (lane < nseg) my_slot = __ldg(g.stat_seg_slot + seg0 + lane);   // lane s: slot of the chunk's segment s
-            if (nseg > 1) {                                // rows of several samples in this chunk: rank of my sample run
-              const int b = row_ok ? (g.stat_sample ? __ldg(g.stat_sample + m) : m / g.stat_rows_per_sample) : -1;
-              const int bp = __shfl_up_sync(0xffffffffu, b, 1);
-              const unsigned chg = __ballot_sync(0xffffffffu, lane > 0 && row_ok && b != bp);
-              my_seg = __popc(chg & (0xffffffffu >> (31 - lane)));
-            }
+      const int m0 = (ptile / p.n_tiles) * TC_BM, n0 = (ptile % p.n_tiles) * BN;
+#pragma unroll
+      for (int i = 0; i < BN / 2; ++i) fence_operand(acc[i]);
+      int prev = 0;
+      for (int kb = 0; kb < p.num_kb; ++kb) {
+        mbar_wait(bar_full + 8 * stage, phase);
+        fence_proxy_async_smem();
+        const uint32_t a_addr = smem_base + stage * Cfg::STAGE_BYTES;
+        const uint64_t da = make_desc_sw128(a_addr + cw * 64 * 128), db = make_desc_sw128(a_addr + Cfg::A_BYTES);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < TC_BK / 16; ++k) Wgmma<BN>::mma(acc, da + 2 * k, db + 2 * k, (kb > 0 || k > 0) ? 1u : 0u);
+        wgmma_commit();
+        wgmma_wait<1>();                                   // the previous stage's MMAs have read their operands
+        if (kb > 0 && t == 0) mbar_arrive(bar_empty + 8 * prev);
+        prev = stage;
+        if (++stage == Cfg::STAGES) { stage = 0; phase ^= 1u; }
+      }
+      wgmma_wait<0>();
+#pragma unroll
+      for (int i = 0; i < BN / 2; ++i) fence_operand(acc[i]);
+      if (t == 0) mbar_arrive(bar_empty + 8 * prev);
+
+      // ---- epilogue: warp (w & 1) owns rows 32 (w & 1) .. +31 of the warpgroup's 64, column half (w >> 1) of each
+      // staged 64-column block; lane = row ----
+      constexpr int CH = BN >= 32 ? 32 : 16;
+      const int rl = (warp & 1) * 32 + lane;
+      const int cc = (warp >> 1) * 32;
+      const bool active = cc < Cfg::EPI_COLS;             // (warp-uniform)
+      const uint32_t stg = epi + (uint32_t)cw * 64 * Cfg::EPI_LD * 4;
+      const int m = m0 + cw * 64 + rl;
+      const bool row_ok = m < g.M;
+      const int64_t orow = row_ok ? (g.out_rows ? (int64_t)g.out_rows[m] : (int64_t)m + split_row0) : 0;
+      const float* radd = (row_ok && g.row_add) ? g.row_add + (int64_t)g.row_add_idx[m] * g.ld_row_add : nullptr;
+      const __nv_bfloat16* res =
+          (row_ok && g.resid) ? reinterpret_cast<const __nv_bfloat16*>(g.resid) + (int64_t)m * g.ld_resid : nullptr;
+      // ---- group-norm partial statistics of this 32-row chunk (see of_gemm_args.stat_out) ----
+      int nseg = 0, my_seg = 0, my_slot = 0;
+      if (active && g.stat_out != nullptr) {
+        const int chunk = (m0 + cw * 64 + (warp & 1) * 32) / 32;
+        if (chunk * 32 < g.M) {
+          const int seg0 = __ldg(g.stat_chunk_seg + chunk);
+          nseg = __ldg(g.stat_chunk_seg + chunk + 1) - seg0;
+          if (lane < nseg) my_slot = __ldg(g.stat_seg_slot + seg0 + lane);   // lane s: slot of the chunk's segment s
+          if (nseg > 1) {                                  // rows of several samples in this chunk: rank of my sample run
+            const int b = row_ok ? (g.stat_sample ? __ldg(g.stat_sample + m) : m / g.stat_rows_per_sample) : -1;
+            const int bp = __shfl_up_sync(0xffffffffu, b, 1);
+            const unsigned chg = __ballot_sync(0xffffffffu, lane > 0 && row_ok && b != bp);
+            my_seg = __popc(chg & (0xffffffffu >> (31 - lane)));
           }
         }
-        // ---- per-column addends (bias + emb[batch]): when the 32 rows of this warp share one sample -- nearly always --
-        // the BN-wide row is staged ONCE per row tile in the warp's shared-memory slot and read back as broadcast
-        // ld.shared.v4 per chunk; per-row global loads (L2 latency on every chunk: the 13 KB of L1 left beside the rings
-        // do not hold them) made the epilogue of the short-K layers longer than their main loop
-        bool staged = false;
-        const uint32_t my_stage = aux + 1024 + ew * 1024;
-        if ((g.bias != nullptr || g.row_add != nullptr) && n0 + BN <= g.N && (g.N % 4 == 0) &&
-            (g.row_add == nullptr || (g.ld_row_add % 4 == 0 && reinterpret_cast<uintptr_t>(g.row_add) % 16 == 0)) &&
-            (g.bias == nullptr || reinterpret_cast<uintptr_t>(g.bias) % 16 == 0)) {
-          const int bsel = (row_ok && g.row_add) ? g.row_add_idx[m] : -1;
-          const int b0 = __shfl_sync(0xffffffffu, bsel, 0);
-          if (__all_sync(0xffffffffu, !row_ok || bsel == b0) && (g.row_add == nullptr || b0 >= 0)) {
-            staged = true;
-            __syncwarp();                                   // the previous row tile's reads of the slot are done
+      }
+      // ---- per-column addends (bias + emb[batch]): when the 32 rows of this warp share one sample -- nearly always --
+      // the BN-wide row is staged ONCE per tile in the warp's shared-memory slot and read back as broadcast ld.shared.v4
+      bool staged = false;
+      const uint32_t my_stage = aux + 1024 + (uint32_t)(cw * 4 + warp) * 1024;
+      if (active && (g.bias != nullptr || g.row_add != nullptr) && n0 + BN <= g.N && (g.N % 4 == 0) &&
+          (g.row_add == nullptr || (g.ld_row_add % 4 == 0 && reinterpret_cast<uintptr_t>(g.row_add) % 16 == 0)) &&
+          (g.bias == nullptr || reinterpret_cast<uintptr_t>(g.bias) % 16 == 0)) {
+        const int bsel = (row_ok && g.row_add) ? g.row_add_idx[m] : -1;
+        const int b0 = __shfl_sync(0xffffffffu, bsel, 0);
+        if (__all_sync(0xffffffffu, !row_ok || bsel == b0) && (g.row_add == nullptr || b0 >= 0)) {
+          staged = true;
+          __syncwarp();                                   // the previous tile's reads of the slot are done
 #pragma unroll
-            for (int i = lane * 4; i < BN; i += 128) {
-              float4 t = make_float4(0.f, 0.f, 0.f, 0.f);
-              if (g.bias) t = __ldg(reinterpret_cast<const float4*>(g.bias + n0 + i));
-              if (g.row_add) {
-                const float4 e = __ldg(reinterpret_cast<const float4*>(g.row_add + (int64_t)b0 * g.ld_row_add + n0 + i));
-                t.x += e.x; t.y += e.y; t.z += e.z; t.w += e.w;
-              }
-              asm volatile("st.shared.v4.f32 [%0], {%1,%2,%3,%4};" ::"r"(my_stage + i * 4), "f"(t.x), "f"(t.y), "f"(t.z), "f"(t.w) : "memory");
+          for (int i = lane * 4; i < BN; i += 128) {
+            float4 tb = make_float4(0.f, 0.f, 0.f, 0.f);
+            if (g.bias) tb = __ldg(reinterpret_cast<const float4*>(g.bias + n0 + i));
+            if (g.row_add) {
+              const float4 e = __ldg(reinterpret_cast<const float4*>(g.row_add + (int64_t)b0 * g.ld_row_add + n0 + i));
+              tb.x += e.x; tb.y += e.y; tb.z += e.z; tb.w += e.w;
             }
-            __syncwarp();
+            asm volatile("st.shared.v4.f32 [%0], {%1,%2,%3,%4};" ::"r"(my_stage + i * 4), "f"(tb.x), "f"(tb.y), "f"(tb.z), "f"(tb.w) : "memory");
+          }
+          __syncwarp();
+        }
+      }
+      // one CH-column chunk of my row: (+bias, +emb, +residual) -> store (+ norm statistics)
+      auto process = [&](float (&v)[32], int c0) {
+        const int nb = n0 + c0;
+        const bool full = (nb + CH <= g.N);
+        if (staged) {
+#pragma unroll
+          for (int q = 0; q < CH / 4; ++q) {
+            float4 tb;
+            asm volatile("ld.shared.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(tb.x), "=f"(tb.y), "=f"(tb.z), "=f"(tb.w) : "r"(my_stage + (c0 + 4 * q) * 4));
+            v[4 * q] += tb.x; v[4 * q + 1] += tb.y; v[4 * q + 2] += tb.z; v[4 * q + 3] += tb.w;
           }
         }
-        constexpr int CH = BN >= 32 ? 32 : 16;
-        // one 32-column chunk of my row: accumulators -> (+bias, +emb, +residual) -> store (+ norm statistics)
-        auto process = [&](uint32_t (&acc)[32], int c0) {
-          const int nb = n0 + c0;
-          float v[32];
+        if (row_ok) {
+          if (g.bias && !staged) {
+            if (full && (reinterpret_cast<uintptr_t>(g.bias) % 16 == 0)) {
 #pragma unroll
-          for (int j = 0; j < CH; ++j) v[j] = __uint_as_float(acc[j]);
-          const bool full = (nb + CH <= g.N);
-          if (staged) {
-#pragma unroll
-            for (int q = 0; q < CH / 4; ++q) {
-              float4 t;
-              asm volatile("ld.shared.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(t.x), "=f"(t.y), "=f"(t.z), "=f"(t.w) : "r"(my_stage + (c0 + 4 * q) * 4));
-              v[4 * q] += t.x; v[4 * q + 1] += t.y; v[4 * q + 2] += t.z; v[4 * q + 3] += t.w;
-            }
-          }
-          if (row_ok) {
-            if (g.bias && !staged) {
-              if (full && (reinterpret_cast<uintptr_t>(g.bias) % 16 == 0)) {
-#pragma unroll
-                for (int q = 0; q < CH / 4; ++q) {
-                  const float4 t = __ldg(reinterpret_cast<const float4*>(g.bias + nb) + q);
-                  v[4 * q] += t.x; v[4 * q + 1] += t.y; v[4 * q + 2] += t.z; v[4 * q + 3] += t.w;
-                }
-              } else {
-#pragma unroll
-                for (int j = 0; j < CH; ++j) if (full || nb + j < g.N) v[j] += g.bias[nb + j];
-              }
-            }
-            if (radd && !staged) {
-              // emb[batch] row: 16-byte loads (the 32 scalar loads per chunk this replaces made the epilogue of the
-              // short-K layers 3x longer than their main loop); the rows of a warp nearly always share one sample, so
-              // these are broadcast hits
-              if (full && (g.ld_row_add % 4 == 0) && (reinterpret_cast<uintptr_t>(g.row_add) % 16 == 0)) {
-#pragma unroll
-                for (int q = 0; q < CH / 4; ++q) {
-                  const float4 t = __ldg(reinterpret_cast<const float4*>(radd + nb) + q);
-                  v[4 * q] += t.x; v[4 * q + 1] += t.y; v[4 * q + 2] += t.z; v[4 * q + 3] += t.w;
-                }
-              } else {
-#pragma unroll
-                for (int j = 0; j < CH; ++j) if (full || nb + j < g.N) v[j] += radd[nb + j];
-              }
-            }
-            if (res) {
-              if (full && (g.ld_resid % 8 == 0)) {
-#pragma unroll
-                for (int q = 0; q < CH / 8; ++q) {
-                  float f[8];
-                  bf16x8_to_f32(ldg_nc_v4(res + nb + q * 8), f);
-#pragma unroll
-                  for (int j = 0; j < 8; ++j) v[q * 8 + j] += f[j];
-                }
-              } else {
-#pragma unroll
-                for (int j = 0; j < CH; ++j) if (nb + j < g.N) v[j] += __bfloat162float(res[nb + j]);
-              }
-            }
-            if (g.out_f32) {
-              float* o = reinterpret_cast<float*>(g.out) + orow * g.ldo + nb;
-              if (full && (g.ldo % 4 == 0)) {
-#pragma unroll
-                for (int q = 0; q < CH / 4; ++q)
-                  *reinterpret_cast<float4*>(o + q * 4) = make_float4(v[q * 4], v[q * 4 + 1], v[q * 4 + 2], v[q * 4 + 3]);
-              } else {
-#pragma unroll
-                for (int j = 0; j < CH; ++j) if (nb + j < g.N) o[j] = v[j];
+              for (int q = 0; q < CH / 4; ++q) {
+                const float4 tb = __ldg(reinterpret_cast<const float4*>(g.bias + nb) + q);
+                v[4 * q] += tb.x; v[4 * q + 1] += tb.y; v[4 * q + 2] += tb.z; v[4 * q + 3] += tb.w;
               }
             } else {
-              __nv_bfloat16* o = reinterpret_cast<__nv_bfloat16*>(g.out) + orow * g.ldo + nb;
-              if (full && (g.ldo % 8 == 0)) {
 #pragma unroll
-                for (int q = 0; q < CH / 8; ++q) *reinterpret_cast<uint4*>(o + q * 8) = f32_to_bf16x8(v + q * 8);
-              } else {
-#pragma unroll
-                for (int j = 0; j < CH; ++j) if (nb + j < g.N) o[j] = __float2bfloat16_rn(v[j]);
-              }
+              for (int j = 0; j < CH; ++j) if (full || nb + j < g.N) v[j] += g.bias[nb + j];
             }
           }
-          if constexpr (CH == 32) {
-            if (nseg > 0 && full) {
-             // (sum, sum of squares) of every GRAN-channel granule of my row; rows beyond M contribute zero.
-             // GRAN = 4 when N is a multiple of 128, else 2 (a 64-channel norm has 2 channels per group) -- a property of
-             // the layer, not of the tile shape, so that the small-M dispatch may run a wide layer on narrow tiles.
-             auto stats = [&](auto gran_c) {
+          if (radd && !staged) {
+            if (full && (g.ld_row_add % 4 == 0) && (reinterpret_cast<uintptr_t>(g.row_add) % 16 == 0)) {
+#pragma unroll
+              for (int q = 0; q < CH / 4; ++q) {
+                const float4 tb = __ldg(reinterpret_cast<const float4*>(radd + nb) + q);
+                v[4 * q] += tb.x; v[4 * q + 1] += tb.y; v[4 * q + 2] += tb.z; v[4 * q + 3] += tb.w;
+              }
+            } else {
+#pragma unroll
+              for (int j = 0; j < CH; ++j) if (full || nb + j < g.N) v[j] += radd[nb + j];
+            }
+          }
+          if (res) {
+            if (full && (g.ld_resid % 8 == 0)) {
+#pragma unroll
+              for (int q = 0; q < CH / 8; ++q) {
+                float f[8];
+                bf16x8_to_f32(ldg_nc_v4(res + nb + q * 8), f);
+#pragma unroll
+                for (int j = 0; j < 8; ++j) v[q * 8 + j] += f[j];
+              }
+            } else {
+#pragma unroll
+              for (int j = 0; j < CH; ++j) if (nb + j < g.N) v[j] += __bfloat162float(res[nb + j]);
+            }
+          }
+          if (g.out_f32) {
+            float* o = reinterpret_cast<float*>(g.out) + orow * g.ldo + nb;
+            if (full && (g.ldo % 4 == 0)) {
+#pragma unroll
+              for (int q = 0; q < CH / 4; ++q)
+                *reinterpret_cast<float4*>(o + q * 4) = make_float4(v[q * 4], v[q * 4 + 1], v[q * 4 + 2], v[q * 4 + 3]);
+            } else {
+#pragma unroll
+              for (int j = 0; j < CH; ++j) if (nb + j < g.N) o[j] = v[j];
+            }
+          } else {
+            __nv_bfloat16* o = reinterpret_cast<__nv_bfloat16*>(g.out) + orow * g.ldo + nb;
+            if (full && (g.ldo % 8 == 0)) {
+#pragma unroll
+              for (int q = 0; q < CH / 8; ++q) *reinterpret_cast<uint4*>(o + q * 8) = f32_to_bf16x8(v + q * 8);
+            } else {
+#pragma unroll
+              for (int j = 0; j < CH; ++j) if (nb + j < g.N) o[j] = __float2bfloat16_rn(v[j]);
+            }
+          }
+        }
+        if constexpr (CH == 32) {
+          if (nseg > 0 && full) {
+            // (sum, sum of squares) of every GRAN-channel granule of my row; rows beyond M contribute zero.
+            // GRAN = 4 when N is a multiple of 128, else 2 (a 64-channel norm has 2 channels per group) -- a property of
+            // the layer, not of the tile shape, so that the small-M dispatch may run a wide layer on narrow tiles.
+            auto stats = [&](auto gran_c) {
               constexpr int GRAN = decltype(gran_c)::value;
               constexpr int NV = 2 * 32 / GRAN;
               float a[NV];
@@ -678,452 +539,44 @@ __global__ void __launch_bounds__(TC_THREADS, 1) gather_gemm_tc_kernel(const __g
 #pragma unroll 1
                 for (int s = 0; s < nseg; ++s) {
                   const int slot = __shfl_sync(0xffffffffu, my_slot, s);
-                  float t[NV];
+                  float tt[NV];
 #pragma unroll
-                  for (int j = 0; j < NV; ++j) t[j] = (my_seg == s) ? a[j] : 0.0f;
-                  warp_reduce_vals<NV>(t, lane);
-                  if (writer) dst[(int64_t)slot * nval] = t[0];
+                  for (int j = 0; j < NV; ++j) tt[j] = (my_seg == s) ? a[j] : 0.0f;
+                  warp_reduce_vals<NV>(tt, lane);
+                  if (writer) dst[(int64_t)slot * nval] = tt[0];
                 }
               }
-             };
-             // (a tile of >= 128 columns divides N: the granule is known at compile time there -- compiling both paths into
-             // the wide kernels cost them registers in this loop, +8 % on the 128-wide layers)
-             if constexpr (BN >= 128) stats(std::integral_constant<int, 4>{});
-             else if (g.N % 128 == 0) stats(std::integral_constant<int, 4>{});
-             else stats(std::integral_constant<int, 2>{});
-            }
+            };
+            if constexpr (BN >= 128) stats(std::integral_constant<int, 4>{});
+            else if (g.N % 128 == 0) stats(std::integral_constant<int, 4>{});
+            else stats(std::integral_constant<int, 2>{});
           }
-        };
-        // two TMEM loads in flight per iteration: the epilogue is latency-bound (tcgen05.ld -> wait -> stores), not
-        // issue-bound, and with the MMA warp no longer waiting on barriers a short-K tile leaves it ~8k cycles
-        // The residual row is the one per-row global read of the epilogue; ncu showed its exposed latency (four 16-byte
-        // loads per chunk, L2 / DRAM) as the largest stall of the epilogue warps.  Holding the next chunks' values in
-        // registers spilled (and slowed every layer); instead the 128-byte line of the NEXT chunk pair is prefetched into
-        // L1 (~30 KB are left beside the rings) one iteration ahead -- no registers, one instruction.
-        auto prefetch_res = [&](int c) {
-          if (res != nullptr && n0 + c < g.N) asm volatile("prefetch.global.L1 [%0];" ::"l"(res + n0 + c));
-        };
-        prefetch_res(chalf * 2 * CH);
-#pragma unroll 1
-        for (int c0 = chalf * 2 * CH; c0 < BN; c0 += (TC_EPI_WARPS / 4) * 2 * CH) {   // (with 8 warps the quarter's other warp takes the chunks between)
-          prefetch_res(c0 + (TC_EPI_WARPS / 4) * 2 * CH);
-          uint32_t accA[32], accB[32];
-          const uint32_t taddr = tmem_base + ((uint32_t)(qw * 32) << 16) + (uint32_t)((as * MT + h) * BN + c0);
-          const bool pair = c0 + CH < BN;
-          if (CH == 32) { OF_TMEM_LD32(taddr, accA); if (pair) { OF_TMEM_LD32(taddr + CH, accB); } }
-          else { OF_TMEM_LD16(taddr, accA); if (pair) { OF_TMEM_LD16(taddr + CH, accB); } }
-          tmem_ld_wait();
-          if (p.debug & 4) continue;
-          process(accA, c0);
-          if (pair) process(accB, c0 + CH);
-        }
-      }
-      tc_fence_before();
-      if (CG == 2 && rank != 0) mbar_arrive_cluster(map_to_cta(bar_tempty + 8 * as, 0));   // the leader issues the MMAs
-      else mbar_arrive(bar_tempty + 8 * as);
-      if (ew == 0 && lane == 0) trace_put(p, 6, tn, tr);
-    }
-  } else if (warp == W.mma) {
-   if (CG == 1 || rank == 0) {
-    // =========================== MMA issuer ===========================
-    // Issuing is nearly synchronous with execution (the tensor pipe accepts only a few MMAs ahead), so every cycle this
-    // warp spends between two MMAs is a cycle the tensor pipe idles; an mbarrier wait costs 100-300 cycles even when the
-    // phase has long completed (profiles/tc_gather_experiments_r02.md).  The full barriers are therefore watched by
-    // the scout warp, which publishes per ring slot the number of completed fills in shared memory; this warp only
-    // reads that word (ld.acquire, ~30 cycles), issues the stage's MMAs from converged code (elect.sync) and commits.
-    constexpr uint32_t idesc = CG == 2 ? make_idesc_pair(BN) : make_idesc(BN);
-    int stage = 0, bstage = 0;
-    uint32_t round = 0, bround = 0;                          // fills of the current slot consumed so far
-    int it = 0, tn = 0;
-    for (int tile = w_first; tile < total_tiles; tile += w_stride, ++it) {
-      const int as = it & 1;
-      mbar_wait(bar_tempty + 8 * as, ((it >> 1) & 1) ^ 1);
-      tc_fence_after();
-      const uint32_t d_tmem = tmem_base + (uint32_t)(as * MT * BN);
-      for (int kb = 0; kb < p.num_kb; kb += KSUB) {
-        if (tr && lane == 0) trace_put(p, 0, tn, true);      // (elect.sync picks lane 0 of the converged warp)
-        {
-          // ready = the slot's fill count has passed the number of fills already consumed (for a pair the leader's scout
-          // counts a fill only when the peer has signalled its half as well)
-          auto ready = [&]() {
-            const uint32_t fa = ld_acquire_cta(flag_a + 4 * stage);
-            const uint32_t fb = U1 ? ~0u : ld_acquire_cta(flag_b + 4 * bstage);
-            return fa > round && (U1 || fb > bround);
-          };
-          if (!ready()) {
-            const long long t0 = clock64();
-            while (!ready()) {
-              if (clock64() - t0 > 4000000000ll) {
-                printf("octfusion_b200 gemm_tc: MMA warp starved (block %d slot %d round %u)\n", (int)blockIdx.x, stage, round);
-                __trap();
-              }
-            }
-          }
-        }
-        const uint32_t a_addr = stage_base + stage * Cfg::STAGE_BYTES;
-        const uint32_t b_addr = U1 ? a_addr + Cfg::A_BYTES : b_ring + bstage * Cfg::B_BYTES;
-        // descriptor low words: start address >> 4 (+2 per 32-byte K step), LBO = 1; the high word is constant
-        const uint32_t a_lo = ((a_addr & 0x3FFFFu) >> 4) | (1u << 16);
-        const uint32_t b_lo = ((b_addr & 0x3FFFFu) >> 4) | (1u << 16);
-        const bool two = KSUB > 1 && kb + 1 < p.num_kb;       // odd K-block count: the last stage is half full
-        if (elect_one()) {
-          trace_put(p, 0, tn, tr);
-          if (!(p.debug & 8)) {
-#pragma unroll
-            for (int j = 0; j < KSUB; ++j) {
-              if (j > 0 && !two) break;
-#pragma unroll
-              for (int k = 0; k < TC_BK / 16; ++k)
-#pragma unroll
-                for (int h = 0; h < MT; ++h) {
-                  if constexpr (CG == 2)
-                    umma_bf16_lo2(d_tmem, a_lo + 2 * k, b_lo + 2 * k, idesc, (kb > 0 || k > 0) ? 1u : 0u);
-                  else
-                    umma_bf16_lo(d_tmem + (uint32_t)(h * BN), a_lo + (j * MT + h) * (Cfg::A_SUB_BYTES >> 4) + 2 * k,
-                                 b_lo + j * (Cfg::B_SUB_BYTES >> 4) + 2 * k, idesc, (kb + j > 0 || k > 0) ? 1u : 0u);
-                }
-            }
-          }
-          trace_put(p, 0, tn, tr);
-          if constexpr (CG == 2) {                       // multicast: the barrier at this offset in BOTH CTAs
-            umma_commit2(bar_empty + 8 * stage);
-            if constexpr (!U1) umma_commit2(bar_bempty + 8 * bstage);
-            if (kb + KSUB >= p.num_kb) umma_commit2(bar_tfull + 8 * as);
-          } else {
-            umma_commit(bar_empty + 8 * stage);            // frees the stage when these MMAs retire
-            if constexpr (!U1) umma_commit(bar_bempty + 8 * bstage);
-            if (kb + KSUB >= p.num_kb) umma_commit(bar_tfull + 8 * as);   // accumulators complete -> epilogue
-          }
-          trace_put(p, 0, tn, tr);
-        }
-        __syncwarp();
-        if (++stage == Cfg::A_STAGES) { stage = 0; ++round; }
-        if constexpr (!U1) { if (++bstage == Cfg::B_STAGES) { bstage = 0; ++bround; } }
-      }
-    }
-   }
-  } else if (warp == W.scout) {
-    // =========================== scout ===========================
-    // One lane per ring slot (lanes 0..A_STAGES-1: gathered tiles, lanes 16..: weight tiles) polls its slot's full
-    // barrier with the non-blocking mbarrier.test_wait -- all slots in one instruction -- and publishes the number of
-    // completed fills of the slot (see the MMA issuer).  A slot cannot complete twice between two polls: the MMA warp
-    // must consume it in between.
-    const int my_tiles = (total_tiles - w_first + w_stride - 1) / w_stride;
-    const uint32_t total_stages = (uint32_t)my_tiles * (uint32_t)((p.num_kb + KSUB - 1) / KSUB);
-    const bool is_a = lane < Cfg::A_STAGES;
-    const bool is_b = !U1 && lane >= 16 && lane < 16 + Cfg::B_STAGES;
-    const uint32_t nslots = is_a ? Cfg::A_STAGES : (Cfg::B_STAGES > 0 ? Cfg::B_STAGES : 1);
-    const uint32_t slot = is_a ? lane : lane - 16;
-    const uint32_t my_total = (is_a || is_b) ? (total_stages + nslots - 1 - slot) / nslots : 0u;
-    const uint32_t bar = is_a ? bar_full + 8 * slot : bar_bfull + 8 * slot;
-    const uint32_t flag = is_a ? flag_a + 4 * slot : flag_b + 4 * slot;
-    // pair: the peer's scout forwards each completed fill to the leader's bar_pfull / bar_pbfull (remote mbarrier
-    // arrive); the leader's scout counts a fill when both its own stage and the peer's have landed
-    const uint32_t pbar = is_a ? bar_pfull + 8 * slot : bar_pbfull + 8 * slot;
-    const uint32_t pbar_remote = CG == 2 ? map_to_cta(pbar, 0) : 0u;
-    uint32_t done = 0, phase = 0;
-    const long long t0 = clock64();
-    while (__any_sync(0xffffffffu, done < my_total)) {
-      bool ok = done < my_total && mbar_test_wait(bar, phase);
-      if (CG == 2 && rank == 0 && ok) ok = mbar_test_wait_cluster(pbar, phase);
-      if (ok) {
-        if (tr && is_a) {                                  // trace region 7: when the scout saw stage (done * slots + slot) full
-          const uint32_t k = done * nslots + slot;
-          if ((int)k < p.trace_cap) p.trace[(size_t)7 * p.trace_cap + k] = (unsigned long long)clock64();
-        }
-        ++done; phase ^= 1u;
-        if (CG == 2 && rank != 0) mbar_arrive_cluster(pbar_remote);
-        else st_release_cta(flag, done);
-      }
-      if (clock64() - t0 > 40000000000ll) {
-        printf("octfusion_b200 gemm_tc: scout timeout (block %d lane %d done %u of %u)\n", (int)blockIdx.x, lane, done, my_total);
-        __trap();
-      }
-    }
-  } else if (warp == W.loader) {
-    // =========================== weight loader ===========================
-    constexpr int NST = U1 ? Cfg::A_STAGES : Cfg::B_STAGES;
-    int stage = 0, tn = 0;
-    uint32_t phase = 0;
-    const uint8_t* wp = reinterpret_cast<const uint8_t*>(g.w);
-    for (int tile = w_first; tile < total_tiles; tile += w_stride) {
-      // a CTA of a pair streams its half of the tile's weight rows
-      const int vtile = g.reverse ? total_tiles - 1 - tile : tile;
-      const int otile = vtile / ksplit;
-      const int n0 = (otile % p.n_tiles) * BN + (int)rank * (BN / CG);
-      const int kb_off = (vtile - otile * ksplit) * p.num_kb;    // first K block of this virtual tile's range
-      for (int kb = 0; kb < p.num_kb; kb += KSUB) {
-        const uint32_t bfull = U1 ? bar_full + 8 * stage : bar_bfull + 8 * stage;
-        mbar_wait((U1 ? bar_empty : bar_bempty) + 8 * stage, phase ^ 1);
-        if (lane == 0) trace_put(p, 1, tn, tr);
-        const uint32_t b_addr = U1 ? stage_base + stage * Cfg::STAGE_BYTES + Cfg::A_BYTES : b_ring + stage * Cfg::B_BYTES;
-        if (elect_one()) {
-          if (p.debug & 2) { mbar_arrive(bfull); }
-          else {
-            const int nk = min(KSUB, p.num_kb - kb);
-            mbar_arrive_expect_tx(bfull, (uint32_t)nk * Cfg::B_SUB_BYTES);
-            for (int j = 0; j < nk; ++j)
-              bulk_g2s(b_addr + j * Cfg::B_SUB_BYTES, wp + ((int64_t)(kb_off + kb + j) * p.npad + n0) * 128, Cfg::B_SUB_BYTES, bfull);
-          }
-        }
-        __syncwarp();
-        if (lane == 0) trace_put(p, 1, tn, tr);
-        if (++stage == NST) { stage = 0; phase ^= 1; }
-      }
-    }
-  } else if (TG && warp >= W.prod0 && warp < W.prod0 + TC_PROD_WARPS) {
-    // =========================== gather producers, TMA ===========================
-    // Each of the 4 producer groups (2 warps) owns every 4th 16 KB sub-tile, one warp per 64-row half; lanes 0..15
-    // gather rows 4l..4l+3 of the half with ONE tile::gather4 each (row coordinates = the four tap-table entries,
-    // -1 = no neighbour = outside the tensor = zeros).  A lane whose rows include a multi-neighbour slot (pre-averaged
-    // row of a_multi, another tensor map) issues four single-row copies instead.  The TMA writes the 128B-swizzled rows
-    // and completes the stage's full barrier by bytes: no address arithmetic, no LDGSTS, 1 instruction per 512 bytes.
-    // (A TMA instruction is warp-uniform: the compiler serialises the lanes, ~16 issues per warp and sub-tile.)
-    const int pw = warp - W.prod0;
-    if (lane < 16) {
-      const int grp = pw >> 1;
-      const int rg = (pw & 1) * 16 + lane;                          // 4-row group of the sub-tile, 0..31
-      const int32_t* __restrict__ tab = g.tap_tab;
-      constexpr int KSTEP = TC_GROUPS / MT;
-      const int h = grp % MT;
-      const int my_tiles = (total_tiles - w_first + w_stride - 1) / w_stride;
-      const uint32_t slots = (uint32_t)((p.num_kb + KSUB - 1) / KSUB * SUBS);
-      const uint32_t slot_total = (uint32_t)my_tiles * slots;
-      struct Pos { int ti, s, kb, cb, tap; };
-      auto vtile_of = [&](int ti) { const int tile = w_first + ti * w_stride; return g.reverse ? total_tiles - 1 - tile : tile; };
-      auto kb_off = [&](int ti) { return (vtile_of(ti) % ksplit) * p.num_kb; };
-      auto norm = [&](Pos& c) {
-        while (c.s >= (int)slots) { c.s -= (int)slots; ++c.ti; c.kb = c.s / MT; c.cb = 0; c.tap = kb_off(c.ti) + c.kb; }
-        while (c.tap >= taps) { c.tap -= taps; ++c.cb; }
-      };
-      auto tile_m0 = [&](int ti) {
-        const int ptile = vtile_of(ti) / ksplit;
-        return (p.n_tiles == 1 ? ptile : ptile / p.n_tiles) * TILE_ROWS + (h + (int)rank) * TC_BM;
-      };
-      auto fetch_taps = [&](const Pos& c, int32_t* t) {
-        const int m = tile_m0(c.ti) + 4 * rg;
-        if (c.cb >= p.cblocks) {                             // node-type block: rows m..m+3 of nt_block
-#pragma unroll
-          for (int i = 0; i < 4; ++i) t[i] = m + i;
-          return;
-        }
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          t[i] = -1;
-          if (m + i < g.M)
-            t[i] = tab != nullptr ? __ldg(tab + ((uint32_t)(m + i) * (uint32_t)taps + (uint32_t)c.tap))
-                                  : (g.in_rows != nullptr ? __ldg(g.in_rows + m + i) : m + i);
         }
       };
-      int32_t tnext[4] = {-1, -1, -1, -1};
-      Pos cur{0, grp, grp / MT, 0, kb_off(0) + grp / MT};
-      norm(cur);
-      if ((uint32_t)grp < slot_total) fetch_taps(cur, tnext);
-      int tn = 0;
-      for (uint32_t sg_slot = (uint32_t)grp; sg_slot < slot_total; sg_slot += TC_GROUPS) {
-        if (lane == 0) trace_put(p, 2 + grp, tn, tr);
-        const int kb = cur.kb;
-        const int cur_cb = cur.cb;
-        const int ch = cur.cb * TC_BK;
-        const int32_t t0 = tnext[0], t1 = tnext[1], t2 = tnext[2], t3 = tnext[3];
-        cur.s += TC_GROUPS; cur.kb += KSTEP; cur.tap += KSTEP;
-        norm(cur);
-        if (sg_slot + TC_GROUPS < slot_total) fetch_taps(cur, tnext);
-        const uint32_t sg = sg_slot / SUBS;
-        const uint32_t stage = sg % Cfg::A_STAGES;
-        const uint32_t phase = (sg / Cfg::A_STAGES) & 1u;
-        mbar_wait(bar_empty + 8 * stage, phase ^ 1);
-        if (lane == 0) trace_put(p, 2 + grp, tn, tr);
-        const uint32_t bar = bar_full + 8 * stage;
-        const uint32_t dst = stage_base + stage * Cfg::STAGE_BYTES + (sg_slot % SUBS) * Cfg::A_SUB_BYTES + rg * 512;
-        const bool data = kb < p.num_kb && !(p.debug & 1);
-        if (!data) {
-          if (lane == 0) mbar_arrive(bar);
-        } else {
-          if (lane == 0) mbar_arrive_expect_tx(bar, (uint32_t)Cfg::A_SUB_BYTES / 2);
-          __syncwarp(0xffffu);
-          if (cur_cb >= p.cblocks) {
-            tma_gather4(dst, &p.tm_nt, 0, t0, t1, t2, t3, bar);
-          } else {
-            const bool first = ch < g.c0;
-            const void* map = first ? (const void*)&p.tm_a0 : (const void*)&p.tm_a1;
-            const int col = first ? ch : ch - g.c0;
-            if (min(min(t0, t1), min(t2, t3)) >= -1) {
-              tma_gather4(dst, map, col, t0, t1, t2, t3, bar);
-            } else {
-              const int32_t tt[4] = {t0, t1, t2, t3};
 #pragma unroll
-              for (int i = 0; i < 4; ++i) {
-                if (tt[i] < -1) tma_row(dst + i * 128, &p.tm_multi, ch, -2 - tt[i], bar);
-                else tma_row(dst + i * 128, map, col, tt[i], bar);
-              }
-            }
-          }
+      for (int blk = 0; blk < BN / Cfg::EPI_COLS; ++blk) {
+        named_bar_sync(1 + cw, 128);                       // the previous block's reads of the staging are done
+#pragma unroll
+        for (int j = 0; j < Cfg::EPI_COLS / 8; ++j) {
+          const int i = blk * (Cfg::EPI_COLS / 2) + 4 * j;
+          const int col = 8 * j + 2 * (lane & 3);
+          const int r0 = warp * 16 + (lane >> 2);
+          asm volatile("st.shared.v2.f32 [%0], {%1,%2};" ::"r"(stg + (uint32_t)(r0 * Cfg::EPI_LD + col) * 4), "f"(acc[i]), "f"(acc[i + 1]) : "memory");
+          asm volatile("st.shared.v2.f32 [%0], {%1,%2};" ::"r"(stg + (uint32_t)((r0 + 8) * Cfg::EPI_LD + col) * 4), "f"(acc[i + 2]), "f"(acc[i + 3]) : "memory");
         }
-        if (lane == 0) trace_put(p, 2 + grp, tn, tr);
-      }
-    }
-  } else if (!TG && warp >= W.prod0 && warp < W.prod0 + TC_PROD_WARPS) {
-    // =========================== gather producers ===========================
-    // 4 independent groups of 2 warps; group g produces the 16 KB sub-tiles whose running index is = g mod 4, so 4
-    // sub-tiles (64 KB of gathers) are in flight per SM and the memory latency of one is hidden behind the other three.
-    // Each thread owns one 16-byte chunk column (q) of 16 rows.
-    const int pt = threadIdx.x - W.prod0 * 32;                      // 0..255
-    const int grp = pt >> 6;                                        // producer group 0..3
-    const int gt = pt & 63;
-    const int q = gt & 7;                                           // 16-byte chunk of the 128-byte row
-    const int rbase = gt >> 3;                                      // 0..7, rows rbase + 8*i
-    const __nv_bfloat16* a0 = reinterpret_cast<const __nv_bfloat16*>(g.a0);
-    const __nv_bfloat16* a1 = reinterpret_cast<const __nv_bfloat16*>(g.a1);
-    const int32_t* __restrict__ tab = g.tap_tab;
-    // Sub-tile slots of a CTA tile in consumption order: slot s -> stage s / SUBS, sub-tile s % SUBS = j * MT + h
-    // (K block (s / SUBS) * KSUB + j of row tile h); padded to whole stages (a pad slot carries no data: its owner only
-    // arrives).  This group owns the slots whose running index over all tiles is = grp (mod 4): its row tile h is fixed
-    // and its K block advances by 4 / MT per iteration.  The 16 table entries of the NEXT owned slot are fetched before
-    // waiting for the current stage to be released, which takes the table latency off the stage turnaround.
-    constexpr int KSTEP = TC_GROUPS / MT;
-    const int h = grp % MT;
-    const int my_tiles = (total_tiles - w_first + w_stride - 1) / w_stride;
-    const uint32_t slots = (uint32_t)((p.num_kb + KSUB - 1) / KSUB * SUBS);
-    const uint32_t slot_total = (uint32_t)my_tiles * slots;
-    // position of a slot inside this CTA's work: (tile iteration, slot, K block, channel block, tap), advanced
-    // incrementally -- no integer divisions in the producer loop (its instruction stream competes with the MMA warp)
-    struct Pos { int ti, s, kb, cb, tap; };
-    auto vtile_of = [&](int ti) { const int tile = w_first + ti * w_stride; return g.reverse ? total_tiles - 1 - tile : tile; };
-    auto kb_off = [&](int ti) { return (vtile_of(ti) % ksplit) * p.num_kb; };
-    auto norm = [&](Pos& c) {
-      // (cb, tap) = the ABSOLUTE K block kb_off + kb of the tile's K range (split-K), kb stays relative to the range
-      while (c.s >= (int)slots) { c.s -= (int)slots; ++c.ti; c.kb = c.s / MT; c.cb = 0; c.tap = kb_off(c.ti) + c.kb; }
-      while (c.tap >= taps) { c.tap -= taps; ++c.cb; }
-    };
-    auto tile_m0 = [&](int ti) {
-      const int ptile = vtile_of(ti) / ksplit;
-      return (p.n_tiles == 1 ? ptile : ptile / p.n_tiles) * TILE_ROWS + (h + (int)rank) * TC_BM;
-    };
-    auto fetch_taps = [&](const Pos& c, int32_t* t) {
-      if (c.cb >= p.cblocks || (p.debug & 32)) return;          // (the node-type block: cb == cblocks)
-      const int m0 = tile_m0(c.ti);
-      if (tab != nullptr) {
-        const uint32_t base = (uint32_t)(m0 + rbase) * (uint32_t)taps + (uint32_t)c.tap;     // < 2^31 (checked on host)
+        named_bar_sync(1 + cw, 128);
+        if (active) {
+          float v[32];
 #pragma unroll
-        for (int i = 0; i < TC_BM / 8; ++i) {
-          const int m = m0 + rbase + 8 * i;
-          t[i] = -1;
-          if (m < g.M) t[i] = __ldg(tab + (base + (uint32_t)(8 * i) * (uint32_t)taps));
-        }
-      } else if (g.in_rows != nullptr) {
-#pragma unroll
-        for (int i = 0; i < TC_BM / 8; ++i) {
-          const int m = m0 + rbase + 8 * i;
-          t[i] = -1;
-          if (m < g.M) t[i] = __ldg(g.in_rows + m);
-        }
-      } else {
-#pragma unroll
-        for (int i = 0; i < TC_BM / 8; ++i) {
-          const int m = m0 + rbase + 8 * i;
-          t[i] = m < g.M ? m : -1;
+          for (int q = 0; q < CH / 4; ++q)
+            asm volatile("ld.shared.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(v[4 * q]), "=f"(v[4 * q + 1]), "=f"(v[4 * q + 2]), "=f"(v[4 * q + 3])
+                         : "r"(stg + (uint32_t)(rl * Cfg::EPI_LD + cc + 4 * q) * 4));
+          process(v, blk * Cfg::EPI_COLS + cc);
         }
       }
-    };
-    int32_t tnext[TC_BM / 8];
-#pragma unroll
-    for (int i = 0; i < TC_BM / 8; ++i) tnext[i] = -1;
-    Pos cur{0, grp, grp / MT, 0, kb_off(0) + grp / MT};
-    norm(cur);
-    if ((uint32_t)grp < slot_total) fetch_taps(cur, tnext);
-    int tn = 0;
-    for (uint32_t sg_slot = (uint32_t)grp; sg_slot < slot_total; sg_slot += TC_GROUPS) {
-      if (gt == 0) trace_put(p, 2 + grp, tn, tr);
-      const int kb = cur.kb;
-      const int cur_cb = cur.cb;
-      const int m0 = tile_m0(cur.ti);
-      int32_t t[TC_BM / 8];
-#pragma unroll
-      for (int i = 0; i < TC_BM / 8; ++i) t[i] = tnext[i];
-      cur.s += TC_GROUPS; cur.kb += KSTEP; cur.tap += KSTEP;
-      norm(cur);                                           // now the position of slot sg_slot + TC_GROUPS
-      if (sg_slot + TC_GROUPS < slot_total) fetch_taps(cur, tnext);
-      const uint32_t sg = sg_slot / SUBS;                  // stage counter; this slot is its sub-tile sg_slot % SUBS
-      const uint32_t stage = sg % Cfg::A_STAGES;
-      const uint32_t phase = (sg / Cfg::A_STAGES) & 1u;
-      mbar_wait(bar_empty + 8 * stage, phase ^ 1);
-      if (gt == 0) trace_put(p, 2 + grp, tn, tr);
-      const uint32_t a_addr = stage_base + stage * Cfg::STAGE_BYTES + (sg_slot % SUBS) * Cfg::A_SUB_BYTES;
-      const bool data = kb < p.num_kb && !(p.debug & 1);
-      if (!data) {
-      } else if (cur_cb < p.cblocks) {
-        const int ch = cur_cb * TC_BK;
-        const __nv_bfloat16* src;
-        int64_t ld;
-        if (ch < g.c0) { src = a0 + ch; ld = g.lda0; } else { src = a1 + (ch - g.c0); ld = g.lda1; }
-        src += q * 8;
-        const __nv_bfloat16* msrc = reinterpret_cast<const __nv_bfloat16*>(g.a_multi) + ch + q * 8;
-        // 16 asynchronous 16-byte global->shared copies back to back (no registers, no waiting):
-        // one neighbour -> its row; none -> zero fill; several -> the pre-averaged row of a_multi.
-        // Branch-free address: one select of (base, stride) + one 32x32+64 multiply-add per copy -- the producers'
-        // instruction stream is what the MMA warp competes with for issue slots.
-        const uint32_t dst0 = a_addr + rbase * 128 + ((q ^ (rbase & 7)) << 4);    // (rbase + 8i) & 7 == rbase & 7
-        const uint64_t sbase = reinterpret_cast<uint64_t>(src), mbase = reinterpret_cast<uint64_t>(msrc);
-        const uint32_t ldb = (uint32_t)ld * 2u, ldmb = (uint32_t)g.ld_multi * 2u;  // row strides in bytes
-        // Multi-neighbour slots only occur on rows of coarse leaves (the first rows of the graph): two thirds of
-        // the tiles have none, and then every copy is max / multiply-add / compare / LDGSTS.
-        int32_t lo = t[0];
-#pragma unroll
-        for (int i = 1; i < TC_BM / 8; ++i) lo = min(lo, t[i]);
-        if (!__any_sync(0xffffffffu, lo < -1)) {
-          if (p.debug & 64) {
-#pragma unroll
-            for (int i = 0; i < TC_BM / 8; ++i) {
-              const int32_t tv = t[i];
-              const uint64_t addr = sbase + (uint64_t)(uint32_t)max(tv, 0) * (uint64_t)ldb;
-              cp_async_16_ca(dst0 + i * 1024, reinterpret_cast<const void*>(addr), tv == -1 ? 0u : 16u);
-            }
-          } else {
-#pragma unroll
-            for (int i = 0; i < TC_BM / 8; ++i) {
-              const int32_t tv = t[i];
-              const uint64_t addr = sbase + (uint64_t)(uint32_t)max(tv, 0) * (uint64_t)ldb;
-              cp_async_16(dst0 + i * 1024, reinterpret_cast<const void*>(addr), tv == -1 ? 0u : 16u);
-            }
-          }
-        } else {
-#pragma unroll
-          for (int i = 0; i < TC_BM / 8; ++i) {
-            const int32_t tv = t[i];
-            const bool multi = tv < -1;
-            const uint32_t idx = multi ? (uint32_t)(-2 - tv) : (uint32_t)(tv < 0 ? 0 : tv);
-            const uint64_t addr = (multi ? mbase : sbase) + (uint64_t)idx * (uint64_t)(multi ? ldmb : ldb);
-            cp_async_16(dst0 + i * 1024, reinterpret_cast<const void*>(addr), tv == -1 ? 0u : 16u);
-          }
-        }
-      } else {
-        // node-type block, precomputed per graph (of_graph_type_block): a plain coalesced copy of rows m0..m0+127
-        const __nv_bfloat16* nb = reinterpret_cast<const __nv_bfloat16*>(g.nt_block) + q * 8;
-#pragma unroll
-        for (int i = 0; i < TC_BM / 8; ++i) {
-          const int rr = rbase + 8 * i;
-          const int m = m0 + rr;
-          cp_async_16(a_addr + rr * 128 + ((q ^ (rr & 7)) << 4), m < g.M ? (const void*)(nb + (int64_t)m * 64) : (const void*)nb,
-                      m < g.M ? 16u : 0u);
-        }
-      }
-      // one counted arrival per thread: for data slots it fires when this thread's cp.asyncs have landed
-      // (cp.async.mbarrier.arrive.noinc, the CUTLASS sm100 cp.async + UMMA protocol); pad slots arrive directly
-      if (data) cp_async_mbar_arrive_noinc(bar_full + 8 * stage);
-      else mbar_arrive(bar_full + 8 * stage);
-      if (gt == 0) trace_put(p, 2 + grp, tn, tr);
     }
   }
-
-  tc_fence_before();
-  __syncthreads();
-  if constexpr (CG == 2) cluster_sync_all();               // no remote arrive / store may hit a CTA that has exited
-  if (warp == W.mma) {
-    tc_fence_after();
-    if constexpr (CG == 2) tmem_dealloc2(tmem_base, Cfg::TMEM_COLS);
-    else tmem_dealloc(tmem_base, Cfg::TMEM_COLS);
-  }
+  __syncthreads();                                         // no CTA exits while its copies are in flight
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1156,101 +609,41 @@ __global__ void pack_weight_tc_kernel(const float* __restrict__ w, int taps, int
   }
 }
 
-
-static int g_mt = -1, g_uni = -1, g_cg = -1, g_layout = -1;   // kernel variant switches (of_tc_config / environment)
-static int g_tg = -1;                                         // 1: TMA gather producers (of_tc_gather_mode / OCTFUSION_TC_TMAG)
-
-// bf16 [rows, cols] tensor with row stride ld (elements) as a TMA tensor map with a 64 x 1 box, 128B swizzle, zero fill
-// outside: the operand of tile::gather4 (and of single-row copies).  cuTensorMapEncodeTiled only encodes -- no device
-// work -- and is fetched from the driver at run time so the library links against cudart only.
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                  const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-static int make_row_map(CUtensorMap* m, const void* base, int64_t cols, int64_t rows, int64_t ld) {
-  static EncodeTiledFn encode = nullptr;
-  if (encode == nullptr) {
-    void* fn = nullptr;
-    cudaDriverEntryPointQueryResult q = cudaDriverEntryPointSymbolNotFound;
-    cudaError_t e = cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &q);
-    if (e != cudaSuccess || q != cudaDriverEntryPointSuccess || fn == nullptr) {
-      set_error("of_gather_gemm_tc: cuTensorMapEncodeTiled is not available from the driver");
-      return OF_E_CUDA;
-    }
-    encode = reinterpret_cast<EncodeTiledFn>(fn);
-  }
-  if (rows <= 0) rows = 1ll << 30;                      // row count unknown to the caller: only valid rows are ever addressed
-  const cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
-  const cuuint64_t strides[1] = {(cuuint64_t)ld * 2u};
-  const cuuint32_t box[2] = {64u, 1u};
-  const cuuint32_t estr[2] = {1u, 1u};
-  CUresult r = encode(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2u, const_cast<void*>(base), dims, strides, box, estr,
-                      CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                      CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) {
-    set_error("of_gather_gemm_tc: cuTensorMapEncodeTiled(cols=%lld rows=%lld ld=%lld) failed: %d", (long long)cols,
-              (long long)rows, (long long)ld, (int)r);
-    return OF_E_CUDA;
-  }
-  return OF_OK;
-}
-static unsigned long long* g_trace = nullptr;
-static int g_trace_cap = 0, g_trace_block = 0;
-
-template <int BN, int MT, int UNI, int CG = 1, int TG = 0, int SK = 0>
+template <int BN>
 static int launch_tc(TcParams& p, cudaStream_t st) {
-  using Cfg = TcCfg<BN, MT, UNI, CG>;
+  using Cfg = TcCfg<BN>;
   // the opt-in to > 48 KB of dynamic shared memory is a per-device attribute of the function
   static bool configured[64] = {};
   int dev = 0;
   cudaGetDevice(&dev);
   if (dev < 0 || dev >= 64 || !configured[dev]) {
-    cudaError_t e = cudaFuncSetAttribute(gather_gemm_tc_kernel<BN, MT, UNI, CG, TG, SK>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         Cfg::SMEM_BYTES);
+    cudaError_t e = cudaFuncSetAttribute(gather_gemm_tc_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES);
     if (e != cudaSuccess) {
       set_error("of_gather_gemm_tc: cudaFuncSetAttribute(%d B): %s", Cfg::SMEM_BYTES, cudaGetErrorString(e));
       return OF_E_CUDA;
     }
     if (dev >= 0 && dev < 64) configured[dev] = true;
   }
-  p.m_tiles = (p.g.M + TC_BM * MT * CG - 1) / (TC_BM * MT * CG);
+  p.m_tiles = (p.g.M + TC_BM - 1) / TC_BM;
   p.n_tiles = p.npad / BN;
   const int total = p.m_tiles * p.n_tiles * p.ksplit;
-  int grid = CG * total < num_sms() ? CG * total : (num_sms() / CG) * CG;
-  {
-    static int lim = -1;                                   // OCTFUSION_TC_GRID: cap the CTA count (experiments)
-    if (lim < 0) { const char* e = getenv("OCTFUSION_TC_GRID"); lim = e ? atoi(e) : 0; }
-    if (lim > 0 && grid > lim) grid = lim;
-  }
-  if constexpr (CG == 2) {
-    if (grid % 2) --grid;
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3((unsigned)grid);
-    cfg.blockDim = dim3(TC_THREADS);
-    cfg.dynamicSmemBytes = Cfg::SMEM_BYTES;
-    cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    cudaError_t e = cudaLaunchKernelEx(&cfg, gather_gemm_tc_kernel<BN, MT, UNI, CG, TG, SK>, p);
-    if (e != cudaSuccess) {
-      set_error("of_gather_gemm_tc (pair): launch: %s", cudaGetErrorString(e));
-      return OF_E_CUDA;
-    }
-  } else {
-    gather_gemm_tc_kernel<BN, MT, UNI, CG, TG, SK><<<grid, TC_THREADS, Cfg::SMEM_BYTES, st>>>(p);
-  }
+  const int grid = total < num_sms() ? total : num_sms();
+  gather_gemm_tc_kernel<BN><<<grid, TC_THREADS, Cfg::SMEM_BYTES, st>>>(p);
   OF_LAUNCH_CHECK("of_gather_gemm_tc");
   return OF_OK;
 }
 
-int check_gemm_args(const of_gemm_args* a, const char* who);
-
-static int env_int(const char* name, int dflt) {
-  const char* e = getenv(name);
-  return e ? atoi(e) : dflt;
+static int launch_tc_bn(int bn, TcParams& p, cudaStream_t st) {
+  switch (bn) {
+    case 256: return launch_tc<256>(p, st);
+    case 128: return launch_tc<128>(p, st);
+    case 64: return launch_tc<64>(p, st);
+    case 32: return launch_tc<32>(p, st);
+    default: return launch_tc<16>(p, st);
+  }
 }
+
+int check_gemm_args(const of_gemm_args* a, const char* who);
 
 }  // namespace of
 
@@ -1277,28 +670,6 @@ extern "C" int of_pack_weight_tc(const float* w_canonical, int32_t taps, int32_t
   pack_weight_tc_kernel<<<grid, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
       w_canonical, taps, c, ntype, N, npad, num_kb, reinterpret_cast<__nv_bfloat16*>(out));
   OF_LAUNCH_CHECK("of_pack_weight_tc");
-  return OF_OK;
-}
-
-extern "C" int of_tc_config(int32_t mt, int32_t uni, int32_t cg, int32_t layout) {
-  if (g_mt < 0) { g_mt = env_int("OCTFUSION_TC_MT", 2); g_uni = env_int("OCTFUSION_TC_UNI", 1); g_cg = env_int("OCTFUSION_TC_CG", 1); }
-  if (g_layout < 0) g_layout = env_int("OCTFUSION_TC_LAYOUT", 0);
-  if (mt == 1 || mt == 2) g_mt = mt;
-  if (uni >= 0 && uni <= 2) g_uni = uni;
-  if (cg == 1 || cg == 2) g_cg = cg;
-  if (layout >= 0 && layout <= 1) g_layout = layout;
-  return OF_OK;
-}
-
-extern "C" int of_tc_gather_mode(int32_t tma) {
-  if (tma == 0 || tma == 1) g_tg = tma;
-  return OF_OK;
-}
-
-extern "C" int of_tc_trace_set(void* buf, int32_t cap_per_region, int32_t block) {
-  g_trace = reinterpret_cast<unsigned long long*>(buf);
-  g_trace_cap = buf ? cap_per_region : 0;
-  g_trace_block = block;
   return OF_OK;
 }
 
@@ -1329,96 +700,39 @@ static int run_tc(const of_gemm_args* args, int ksplit, void* stream) {
   }
   if (a.M == 0) return OF_OK;
   TcParams p;
-  memset(&p.tm_a0, 0, 4 * sizeof(CUtensorMap));
   p.g = a;
-  {
-    static int dbg = -1;
-    if (dbg < 0) dbg = env_int("OCTFUSION_TC_DEBUG", 0);
-    p.debug = dbg;
-  }
-  p.trace = g_trace; p.trace_cap = g_trace_cap; p.trace_block = g_trace_block;
-  if (g_layout < 0) g_layout = env_int("OCTFUSION_TC_LAYOUT", 0);
-  p.layout = g_layout;
   p.cblocks = (a.c0 + a.c1) / 64;
   p.num_kb = p.cblocks * a.taps + (a.ntype > 0 ? 1 : 0);
   p.ksplit = 1;
   p.npad = (a.N + 15) / 16 * 16;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  // experiment switches (tools/exp_tc.sh): OCTFUSION_TC_MT = row tiles per CTA for the narrow layers (1 | 2),
-  // OCTFUSION_TC_UNI = 1: weight tile in the gather ring's stage (one barrier pair per stage)
-  if (g_mt < 0) { g_mt = env_int("OCTFUSION_TC_MT", 2); g_uni = env_int("OCTFUSION_TC_UNI", 1); g_cg = env_int("OCTFUSION_TC_CG", 1); }
-  const int mt = g_mt, uni = g_uni;
   if (ksplit > 1) {
     OF_REQUIRE(p.num_kb % ksplit == 0 && p.npad % 32 == 0 && a.N == p.npad && a.out_rows == nullptr && a.out_f32 == 1 &&
                    a.bias == nullptr && a.row_add == nullptr && a.resid == nullptr && a.stat_out == nullptr,
                "of_gather_gemm_tc_splitk: internal argument error");
     p.ksplit = ksplit;
     p.num_kb /= ksplit;
-    // one 128-row tile per CTA: the point is many short K loops
-    if (p.npad % 256 == 0) return launch_tc<256, 1, 1, 1, 0, 1>(p, st);
-    if (p.npad % 128 == 0) return launch_tc<128, 1, 0, 1, 0, 1>(p, st);
-    if (p.npad % 64 == 0) return launch_tc<64, 1, 0, 1, 0, 1>(p, st);
-    return launch_tc<32, 1, 0, 1, 0, 1>(p, st);
+    return launch_tc_bn(p.npad % 256 == 0 ? 256 : p.npad % 128 == 0 ? 128 : p.npad % 64 == 0 ? 64 : 32, p, st);
   }
-  if (g_tg < 0) g_tg = env_int("OCTFUSION_TC_TMAG", 0);
-  if (g_tg == 1 && a.lda0 % 64 == 0 && (a.c1 == 0 || a.lda1 % 64 == 0) && reinterpret_cast<uintptr_t>(a.a0) % 128 == 0 &&
-      reinterpret_cast<uintptr_t>(a.a1) % 128 == 0 && (a.a_multi == nullptr || a.ld_multi % 64 == 0)) {
-    // TMA gather producers (128-byte aligned rows): tensor maps of the operands
-    if ((rc = make_row_map(&p.tm_a0, a.a0, a.c0, a.rows_a0, a.lda0))) return rc;
-    if (a.c1 > 0) { if ((rc = make_row_map(&p.tm_a1, a.a1, a.c1, a.rows_a1, a.lda1))) return rc; }
-    else p.tm_a1 = p.tm_a0;
-    if (a.a_multi != nullptr) { if ((rc = make_row_map(&p.tm_multi, a.a_multi, a.c0 + a.c1, 0, a.ld_multi))) return rc; }
-    else p.tm_multi = p.tm_a0;
-    if (a.ntype > 0) { if ((rc = make_row_map(&p.tm_nt, a.nt_block, 64, a.M, 64))) return rc; }
-    else p.tm_nt = p.tm_a0;
-    if (p.npad % 256 == 0) return launch_tc<256, 1, 1, 1, 1>(p, st);
-    if (p.npad % 128 == 0) return launch_tc<128, 2, 1, 1, 1>(p, st);
-    if (p.npad % 64 == 0) return launch_tc<64, 2, 0, 1, 1>(p, st);
-    if (p.npad % 32 != 0) return launch_tc<16, 2, 0, 1, 1>(p, st);
-  }
+  if (p.npad % 32 != 0) return launch_tc<16>(p, st);
   // Small M (the dense 4^3 / 8^3 levels: 2048 / 16384 rows): the widest tile would leave most SMs idle (16 row tiles of 128
-  // rows for 148 SMs) with every CTA walking the whole K loop alone.  Take the widest tile shape whose tile count still
+  // rows for 132 SMs) with every CTA walking the whole K loop alone.  Take the widest tile shape whose tile count still
   // fills 3/4 of the SMs, else the shape with the most tiles: narrower column tiles re-gather the (L2-resident) rows but
   // split the weight stream and the MMAs over more SMs.  (The statistics granule follows N, not the tile shape.)
-  if (g_cg != 2 && mt == 2 && p.npad % 32 == 0) {
-    struct Shape { int bn, mt; };
-    static const Shape shapes[] = {{256, 1}, {128, 2}, {128, 1}, {64, 2}, {64, 1}, {32, 2}, {32, 1}};
-    auto tiles = [&](const Shape& sh) { return (int64_t)((a.M + 128 * sh.mt - 1) / (128 * sh.mt)) * (p.npad / sh.bn); };
-    int best = -1;
-    int64_t best_tiles = -1;
-    const int64_t enough = (int64_t)num_sms() * 3 / 4;
-    for (int i = 0; i < 7; ++i) {
-      const Shape& sh = shapes[i];
-      if (p.npad % sh.bn != 0) continue;
-      const int64_t t = tiles(sh);
-      if (best < 0) { best = i; best_tiles = t; }            // the default: the widest shape that divides N
-      if (best_tiles >= enough) break;
-      if (t > best_tiles) { best = i; best_tiles = t; }
-      if (t >= enough) break;
-    }
-    if (best >= 2) {                                         // (0, 1 = the defaults handled below)
-      switch (best) {
-        case 2: return launch_tc<128, 1, 0>(p, st);
-        case 3: return launch_tc<64, 2, 0>(p, st);
-        case 4: return launch_tc<64, 1, 0>(p, st);
-        case 5: return launch_tc<32, 2, 0>(p, st);
-        default: return launch_tc<32, 1, 0>(p, st);
-      }
-    }
-    if (best == 1 && p.npad % 256 == 0) return uni == 1 ? launch_tc<128, 2, 1>(p, st) : launch_tc<128, 2, 0>(p, st);
+  static const int widths[] = {256, 128, 64, 32};
+  const int64_t row_tiles = (a.M + TC_BM - 1) / TC_BM;
+  const int64_t enough = (int64_t)num_sms() * 3 / 4;
+  int bn = 0;
+  int64_t best_tiles = -1;
+  for (int w : widths) {
+    if (p.npad % w != 0) continue;
+    const int64_t t = row_tiles * (p.npad / w);
+    if (bn == 0) { bn = w; best_tiles = t; }              // the default: the widest shape that divides N
+    if (best_tiles >= enough) break;
+    if (t > best_tiles) { bn = w; best_tiles = t; }
+    if (t >= enough) break;
   }
-  // widest tile that divides the padded N: fewer re-gathers of A per output column
-  if (p.npad % 256 == 0) {
-    if (g_cg == 2 && a.M > 256) return uni == 2 ? launch_tc<256, 1, 2, 2>(p, st) : launch_tc<256, 1, 0, 2>(p, st);
-    return uni == 1 ? launch_tc<256, 1, 1>(p, st) : uni == 2 ? launch_tc<256, 1, 2>(p, st) : launch_tc<256, 1, 0>(p, st);
-  }
-  if (p.npad % 128 == 0) {
-    if (mt == 1) return launch_tc<128, 1, 0>(p, st);
-    return uni == 1 ? launch_tc<128, 2, 1>(p, st) : launch_tc<128, 2, 0>(p, st);
-  }
-  if (p.npad % 64 == 0) return launch_tc<64, 2, 0>(p, st);
-  if (p.npad % 32 == 0) return launch_tc<32, 2, 0>(p, st);
-  return launch_tc<16, 2, 0>(p, st);
+  return launch_tc_bn(bn, p, st);
 }
 
 extern "C" int of_gather_gemm_tc(const of_gemm_args* args, void* stream) { return run_tc(args, 1, stream); }
@@ -1508,9 +822,6 @@ static int splitk_plan(const of_gemm_args& a) {
   if (a.dtype != OF_BF16 || a.c0 % 64 != 0 || a.c1 % 64 != 0 || a.N % 32 != 0 || a.out_rows != nullptr || a.M <= 0 ||
       a.a_silu || (a.ntype > 0 && a.nt_block == nullptr))
     return 1;
-  if (g_cg < 0) g_cg = env_int("OCTFUSION_TC_CG", 1);
-  if (g_tg < 0) g_tg = env_int("OCTFUSION_TC_TMAG", 0);
-  if (g_cg == 2 || g_tg == 1) return 1;
   const int num_kb = (a.c0 + a.c1) / 64 * a.taps + (a.ntype > 0 ? 1 : 0);
   const int bn = a.N % 256 == 0 ? 256 : a.N % 128 == 0 ? 128 : a.N % 64 == 0 ? 64 : 32;
   const int64_t tiles = (int64_t)((a.M + 127) / 128) * (a.N / bn);

@@ -344,7 +344,7 @@ __global__ void multi_index_kernel(const int32_t* __restrict__ tab, const int32_
   multi_types[ord] = packed;
 }
 
-// Node-type K block of the tcgen05 GEMM, precomputed once per graph: row m, column tap*ntype + type holds
+// Node-type K block of the tensor-core GEMM, precomputed once per graph: row m, column tap*ntype + type holds
 // (#neighbours of that type in slot (m, tap)) / (#neighbours) = the mean of the one-hot columns the reference
 // appends to the features (modules.py:199-202) -- a graph constant, so the GEMM streams it like any other A tile
 // instead of chasing tap table -> node_type for every tile.

@@ -4,7 +4,7 @@
 // scatter_add passes, two index_select passes and six elementwise passes = ~12 HBM round trips)
 // and the dense GroupNorm32 (modules.py:26-28) by
 //   of_gn_stats     one read  of x            -> per (32-row segment, 4-channel granule) sum / sum of squares in fp32,
-//                   no atomics (bit-reproducible); skipped when the producing tcgen05 GEMM wrote the partials itself
+//                   no atomics (bit-reproducible); skipped when the producing tensor-core GEMM wrote the partials itself
 //   of_gn_finalize  partials summed in fixed order in fp64 -> [B, C] scale / shift table (fp32 result)
 //   of_gn_apply     one read + one write      -> y = SiLU(x * scale + shift), concat fused
 // HBM-bound kernels: 16-byte vector accesses, grid sized in multiples of the SM count.
@@ -87,7 +87,7 @@ __device__ __forceinline__ bool chunk_is_uniform(const GnSrc& s, int64_t r0, int
 }
 
 // Deterministic partial statistics: one thread per (32-row chunk, channel vector) adds its rows in order and writes
-// (sum, sum of squares) per 4-channel granule into the slot of the chunk's segment -- the layout the tcgen05 GEMM
+// (sum, sum of squares) per 4-channel granule into the slot of the chunk's segment -- the layout the tensor-core GEMM
 // epilogue produces (of_gemm_args.stat_out), so of_gn_finalize serves both.  A new segment starts at every change
 // of sample id inside the chunk.
 template <typename T, int V, int GRAN>

@@ -13,10 +13,10 @@ void set_error(const char* fmt, ...) {
 int num_sms() {
   static int cached[64] = {0};
   int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 148;
+  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 132;
   if (!cached[dev]) {
     int n = 0;
-    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 148;
+    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;
     cached[dev] = n;
   }
   return cached[dev];
@@ -27,7 +27,7 @@ void add_launches(int n) { __atomic_fetch_add(&g_launches, (unsigned long long)n
 
 extern "C" unsigned long long of_launch_count(void) { return __atomic_load_n(&of::g_launches, __ATOMIC_RELAXED); }
 extern "C" const char* of_last_error(void) { return of::g_err; }
-extern "C" int of_version(void) { return 4; }
+extern "C" int of_version(void) { return 5; }
 extern "C" int of_abi_sizeof_gemm_args(void) { return (int)sizeof(of_gemm_args); }
 extern "C" int of_abi_sizeof_octree_levels(void) { return (int)sizeof(of_octree_levels); }
 extern "C" int of_num_sms(void) { return of::num_sms(); }

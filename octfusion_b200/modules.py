@@ -1,6 +1,6 @@
 """Drop-in operator classes: same names, constructor signatures, forward signatures and
 state_dict keys as reference models/networks/modules.py (SURVEY.md 8b), every forward executed by
-the sm_100a kernels of liboctfusion_b200.so.  Inference only (the hot path is the sampler's
+the sm_90a kernels of liboctfusion_b200.so.  Inference only (the hot path is the sampler's
 per-step U-Net forward); no autograd through the custom kernels.
 
 Sparse (dual-octree) tensors are [N_d, C] row-major exactly as in the reference.  Dense (LR middle
@@ -61,7 +61,7 @@ class GraphConv(nn.Module):
         return self._pw.refresh(self.weights, 'canon')
 
     def prepared_padded(self, cpad=64):
-        """weights re-laid for an input zero-padded to `cpad` channels (tcgen05 path needs C % 64 == 0; the
+        """weights re-laid for an input zero-padded to `cpad` channels (tensor-core path needs C % 64 == 0; the
         3- or 8-channel latent of the first conv is padded instead of falling back to the CUDA cores)."""
         key = (self.weights.data_ptr(), self.weights._version)
         if getattr(self, '_pw_pad_key', None) != key:

@@ -98,7 +98,7 @@ class OctreeConv(nn.Module):
         tap = TapTable(neigh, None, 27)
         x = data.contiguous()
         if x.dtype == torch.bfloat16 and self.in_channels % 64 != 0:
-            # tcgen05 path wants 64-channel slabs: zero-pad the (narrow) input instead of leaving the tensor cores
+            # tensor-core path wants 64-channel slabs: zero-pad the (narrow) input instead of leaving the tensor cores
             cpad = (self.in_channels + 63) // 64 * 64
             xp = torch.zeros((x.shape[0], cpad), dtype=x.dtype, device=x.device)
             ops.copy_rows(x, xp, x.shape[0], self.in_channels)

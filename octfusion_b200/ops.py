@@ -46,7 +46,7 @@ def set_force_simt(flag: bool):
 class TapTable:
     """Neighbour table of the tap-gather GEMM (see include/octfusion_b200.h).
     tab/extra: record encoding (CUDA-core path).  tab_ord/multi_off/multi_types: ordinal encoding of the
-    multi-neighbour slots for the tcgen05 path (of_graph_multi_index); n_multi = number of such slots."""
+    multi-neighbour slots for the tensor-core path (of_graph_multi_index); n_multi = number of such slots."""
     __slots__ = ('tab', 'extra', 'taps', 'rows', 'tab_ord', 'multi_off', 'multi_types', 'n_multi', '_type_blocks', '_scan')
 
     def __init__(self, tab: torch.Tensor, extra, taps: int):
@@ -58,7 +58,7 @@ class TapTable:
         self._scan = None
 
     def type_block(self, ntype, node_type):
-        """bf16 [rows, 64] node-type K block of the tcgen05 GEMM (graph constant, built once per ntype)."""
+        """bf16 [rows, 64] node-type K block of the tensor-core GEMM (graph constant, built once per ntype)."""
         if ntype not in self._type_blocks:
             out = torch.empty((self.rows, 64), dtype=torch.bfloat16, device=self.tab.device)
             check(lib.of_graph_type_block(ptr(self.tab), ptr(self.extra), ptr(node_type), self.rows, self.taps, ntype,
@@ -170,7 +170,7 @@ class StatPlan:
 
 
 def tc_stat_gran(n: int) -> int:
-    """granule width of the statistics the tcgen05 epilogue writes for an N-column output (gemm_tc.cu: 4 for the
+    """granule width of the statistics the tensor-core epilogue writes for an N-column output (gemm_tc.cu: 4 for the
     128/256-wide tiles, 2 below -- a 64-channel GroupNorm32 has 2 channels per group)"""
     return 4 if n % 128 == 0 else 2
 
@@ -184,15 +184,15 @@ class Stats:
 
 
 _FUSE_STATS = os.environ.get('OCTFUSION_GN_FUSE', '1') != '0'     # 0: always run the stand-alone statistics pass
-# split-K for small-M tcgen05 GEMMs (of_gather_gemm_tc_splitk): opt-in.  Measured -0.17 ms per step, but the different
-# rounding pattern moves the bf16 max-norm error of the dense LR nets by +-5 %, and those parity tests sit at their
-# tolerance (1.94e-2 of 2e-2): the default keeps the single-pass kernel with the small-M tile dispatch.
+# split-K for small-M tensor-core GEMMs (of_gather_gemm_tc_splitk): opt-in.  It sums K in another order than the
+# single-pass kernel, so its results differ in the last bits; the default keeps the single-pass kernel with the small-M
+# tile dispatch.  Its effect on the step time was not measured on H100.
 _SPLIT_K = os.environ.get('OCTFUSION_TC_SPLITK', '0') == '1'
 
 
 class PreparedWeight:
     """A GEMM weight in the two layouts the kernels read:
-    canonical fp32 [taps*(c+ntype), N] (CUDA-core path) and the bf16 swizzled tile image (tcgen05
+    canonical fp32 [taps*(c+ntype), N] (CUDA-core path) and the bf16 swizzled tile image (tensor-core
     path, built lazily by of_pack_weight_tc).  Rebuilt when the source parameter changes."""
 
     def __init__(self, taps: int, c: int, ntype: int, n: int):
@@ -237,7 +237,7 @@ class PreparedWeight:
         if self._packed is None:
             nbytes = lib.of_pack_weight_tc_bytes(self.taps, self.c, self.ntype, self.n)
             if nbytes <= 0:
-                raise RuntimeError('weight shape not packable for the tcgen05 path')
+                raise RuntimeError('weight shape not packable for the tensor-core path')
             buf = torch.empty(nbytes, dtype=torch.uint8, device=self.canon.device)
             check(lib.of_pack_weight_tc(ptr(self.canon), self.taps, self.c, self.ntype, self.n, ptr(buf), stream()),
                   'of_pack_weight_tc')
@@ -249,7 +249,7 @@ def gather_gemm(a0, w: PreparedWeight, *, a1=None, tap: TapTable = None, in_rows
                 a_silu=False, bias=None, row_add=None, row_add_idx=None, resid=None, out_rows=None,
                 out=None, ldo=None, out_f32=False, m=None, force_simt=False, stats: StatPlan = None):
     """out[m,:] = sum_tap mean_nbr [a0|a1|onehot] . W[tap] + bias + row_add[row_add_idx[m]] + resid[m].
-    stats: the StatPlan of the output rows when a group norm consumes the output next -- the tcgen05 epilogue then
+    stats: the StatPlan of the output rows when a group norm consumes the output next -- the tensor-core epilogue then
     writes the norm's partial statistics (attached to the result as `_of_stats`), and ops.group_norm skips its
     statistics pass."""
     _lib.require_cuda(a0, a1, bias, row_add, resid, out)
@@ -413,7 +413,7 @@ def _stats_of(x, plan: StatPlan, cpg: int):
 
 def group_norm(x0, gamma, beta, groups: int, plan: StatPlan, *, x1=None, eps=1e-5, count_eps=0.0, act=False, out=None):
     """(x0|x1) -> act(groupnorm) with per-sample statistics over the row layout `plan` describes.  Statistics:
-    deterministic fp32 partials per (32-row segment, 4 channels) -- written by the producing tcgen05 GEMM's epilogue
+    deterministic fp32 partials per (32-row segment, 4 channels) -- written by the producing tensor-core GEMM's epilogue
     when it was asked to (`gather_gemm(stats=plan)`), else by of_gn_stats -- summed in fixed order in fp64."""
     _lib.require_cuda(x0, x1, gamma, beta, out)
     rows = x0.shape[0]

@@ -49,7 +49,7 @@ class HRStepper:
 
     def _weights_key(self):
         """fingerprint of every parameter of the two nets: the captured graph bakes in device copies of the weights
-        (packed tcgen05 images, concatenated embedding projections, padded first conv), so an in-place update, a
+        (packed tensor-core images, concatenated embedding projections, padded first conv), so an in-place update, a
         load_state_dict or an EMA swap must force a re-capture"""
         key = []
         for net in (self.hr, self.lr):

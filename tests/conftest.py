@@ -8,17 +8,12 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line('markers', 'gpu: needs a CUDA device (run on the B200 box with -m gpu)')
-    config.addinivalue_line('markers', 'reference: needs the reference tree at /root/reference (build container only)')
+    config.addinivalue_line('markers', 'gpu: needs a CUDA device (run on an H100 with -m gpu)')
 
 
 def pytest_collection_modifyitems(config, items):
     import torch
     has_gpu = torch.cuda.is_available()
-    from oracle import ref_import
-    has_ref = ref_import.available()
     for it in items:
         if 'gpu' in it.keywords and not has_gpu:
             it.add_marker(pytest.mark.skip(reason='no CUDA device'))
-        if 'reference' in it.keywords and not has_ref:
-            it.add_marker(pytest.mark.skip(reason='reference tree not present'))

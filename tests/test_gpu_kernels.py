@@ -104,66 +104,6 @@ def test_graphconv_bf16_simt_equals_tc():
     assert relerr(y_tc, y_si) < 8e-3
 
 
-@pytest.fixture
-def pair_variant():
-    """run the tcgen05 GEMM's 256-wide tiles as CTA pairs (tcgen05.mma.cta_group::2) for the duration of a test"""
-    from octfusion_b200._lib import lib
-    lib.of_tc_config(-1, -1, 2, -1)
-    yield
-    lib.of_tc_config(-1, -1, 1, -1)
-
-
-@pytest.mark.parametrize('d,cin,cout,nt', [(4, 256, 512, 3), (5, 128, 256, 4), (6, 128, 256, 5), (5, 768, 256, 4)])
-def test_graphconv_bf16_cta_pair(pair_variant, d, cin, cout, nt):
-    """cta_group::2: two CTAs compute one 256-row tile, each gathering its 128 rows and streaming half of the weight
-    tile; same result as the oracle (and the row count of these graphs is not a multiple of 256: the last pair tile
-    has a masked half)."""
-    y, ref32, refbf = _graphconv_case(2, d, cin, cout, nt, torch.bfloat16)
-    assert relerr(y, refbf) < 8e-3
-    assert relerr(y, ref32) < 2e-2
-
-
-def test_cta_pair_equals_single_cta_bitwise(pair_variant):
-    """same MMA order per output element (K blocks in order, fp32 accumulation in TMEM): the pair variant reproduces
-    the single-CTA result bit for bit, epilogue extras and norm statistics included"""
-    from octfusion_b200._lib import lib
-    from octfusion_b200.modules import GraphConv
-    doc = product_doctree(3, 5)
-    d, cin, cout = 5, 256, 256
-    plan = doc.plan[d]
-    conv = GraphConv(cin, cout, 7, 7, d - 1).to(DEV)
-    x = _rand((plan.rows, cin), 3).to(DEV).bfloat16()
-    res = _rand((plan.rows, cout), 4).to(DEV).bfloat16()
-    emb = _rand((3, cout), 5).to(DEV)
-    run = lambda: conv.run(x, plan, row_add=emb, row_add_idx=plan.batch_id, resid=res, stats=plan.stat)  # noqa: E731
-    a = run()
-    lib.of_tc_config(-1, -1, 1, -1)
-    b = run()
-    assert torch.equal(a, b) and torch.equal(a._of_stats.part, b._of_stats.part)
-
-
-@pytest.fixture
-def tma_gather():
-    """fill the gathered operand tiles with the TMA (cp.async.bulk.tensor tile::gather4) for the duration of a test"""
-    from octfusion_b200._lib import lib
-    lib.of_tc_gather_mode(1)
-    yield
-    lib.of_tc_gather_mode(0)
-
-
-@pytest.mark.parametrize('d,cin,cout,nt', [(4, 256, 512, 3), (6, 128, 128, 5), (6, 64, 8, 5), (5, 768, 64, 4)])
-def test_graphconv_bf16_tma_gather_equals_cp_async_bitwise(tma_gather, d, cin, cout, nt):
-    """tile::gather4 producers: a missing neighbour is a row coordinate outside the tensor (zero fill), multi-neighbour
-    slots come from the mean-row tensor map, the node-type block from its own map -- same bytes in shared memory as the
-    cp.async producers, hence the same result bit for bit"""
-    from octfusion_b200._lib import lib
-    y, ref32, refbf = _graphconv_case(2, d, cin, cout, nt, torch.bfloat16)
-    lib.of_tc_gather_mode(0)
-    y0, _, _ = _graphconv_case(2, d, cin, cout, nt, torch.bfloat16)
-    assert relerr(y, refbf) < 8e-3
-    assert torch.equal(y, y0)
-
-
 # ------------------------------------------------------------------------------------------------
 # plain GEMMs with the fused epilogues
 # ------------------------------------------------------------------------------------------------
@@ -279,7 +219,7 @@ def _nan_parts(monkeypatch):
 
 @pytest.mark.parametrize('d,cin,cout,resid', [(6, 128, 128, True), (5, 128, 256, False), (4, 256, 512, False), (6, 64, 64, False)])
 def test_gemm_epilogue_statistics(monkeypatch, d, cin, cout, resid):
-    """The tcgen05 epilogue's group-norm partials (of_gemm_args.stat_out) against the stand-alone of_gn_stats pass over
+    """The tensor-core epilogue's group-norm partials (of_gemm_args.stat_out) against the stand-alone of_gn_stats pass over
     the same output: same slots, sums equal up to the bf16 rounding of the stored tensor; the norm built on either is
     the oracle's norm of the output.  3 ragged samples (chunks that straddle samples take the masked path)."""
     from octfusion_b200 import ops
@@ -415,7 +355,7 @@ def test_linear_small(b, k, n):
 
 
 def test_graphconv_small_channel_input_padded_to_tc():
-    """the 3- / 8-channel latent of the first conv is zero-padded to 64 channels for the tcgen05 path."""
+    """the 3- / 8-channel latent of the first conv is zero-padded to 64 channels for the tensor-core path."""
     for cin in (3, 8):
         y, ref32, refbf = _graphconv_case(2, 6, cin, 128, 5, torch.bfloat16)
         assert relerr(y, refbf) < 8e-3 and relerr(y, ref32) < 2e-2

@@ -167,7 +167,7 @@ def test_unet_against_reference_golden(name, dtype, tol):
     ts = torch.tensor(UNET_TS)[:batch]
     label = torch.tensor(UNET_LABEL)[:batch].to(DEV) if cfg.get('num_classes') else None
     y = net(unet_type='hr', x=x.to(DEV).to(dtype), doctree=doc, timesteps=ts.to(DEV), unet_lr=net.unet_lr, label=label)
-    e = relerr(y.cpu(), torch.from_numpy(g['y']))
+    e = relerr(y.cpu()[::int(g['row_step']) if 'row_step' in g else 1], torch.from_numpy(g['y']))
     print('ERR golden %s %s %.3e' % (name, str(dtype), e))
     assert e < tol, e
 
@@ -175,16 +175,15 @@ def test_unet_against_reference_golden(name, dtype, tol):
 def test_graph_and_config1_against_reference_golden():
     import os
     import numpy as np
-    from tests.util import GOLDEN
+    from tests.util import GOLDEN, digest
     from octfusion_b200.modules import GraphConv
     doc = product_doctree(1, 0)
     g = np.load(os.path.join(GOLDEN, 'dual_graph_b1_s0.npz'))
     for d in range(4, 7):
         k, c = R.edge_set({'edge_idx': doc.graph[d]['edge_idx'].cpu(), 'edge_dir': doc.graph[d]['edge_dir'].cpu()})
-        assert np.array_equal(k.numpy(), g['key%d' % d].astype(np.int64))
-        assert np.array_equal(c.numpy(), g['col%d' % d].astype(np.int64))
-        assert np.array_equal(doc.plan[d].node_type.cpu().numpy(), g['node_type%d' % d])
-        assert np.array_equal(doc.plan[d].batch_id.cpu().numpy(), g['batch_id%d' % d])
+        assert digest(k) == g['key%d' % d] and digest(c) == g['col%d' % d]
+        assert digest(doc.plan[d].node_type) == g['node_type%d' % d]
+        assert digest(doc.plan[d].batch_id) == g['batch_id%d' % d]
     g = np.load(os.path.join(GOLDEN, 'graphconv_config1.npz'))
     conv = GraphConv(8, 8, 7, 7, 0)
     conv.weights.data.copy_(torch.from_numpy(g['w']))

@@ -10,7 +10,7 @@ import pytest
 import torch
 
 from tests.util import UNCOND, COND, SMALL, model_shapes
-from oracle import restate as R, ref_import
+from oracle import restate as R
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
@@ -25,7 +25,7 @@ def test_library_exports_every_declared_symbol():
     for name in declared:
         assert hasattr(lib, name), 'library does not export %s' % name
     assert declared == set(_lib.EXPORTED_SYMBOLS), declared ^ set(_lib.EXPORTED_SYMBOLS)
-    assert lib.of_version() == 4
+    assert lib.of_version() == 5
 
 
 def test_argument_validation_without_gpu():
@@ -39,7 +39,7 @@ def test_argument_validation_without_gpu():
 
 
 def test_splitk_plan_host_logic():
-    """of_tc_splitk_plan is pure host arithmetic (148 SMs assumed without a device): split only launches whose 128-row
+    """of_tc_splitk_plan is pure host arithmetic (132 SMs assumed without a device): split only launches whose 128-row
     tiles cannot fill half of the SMs, into whole K blocks, at least 4 per range, at most one wave of CTAs"""
     from octfusion_b200 import _lib
     def plan(m, n, c, taps, ntype=0, out_rows=None):
@@ -47,16 +47,16 @@ def test_splitk_plan_host_logic():
         g.M, g.N, g.c0, g.c1, g.taps, g.ntype, g.dtype = m, n, c, 0, taps, ntype, 1          # dtype 1 = bf16
         g.out_rows = out_rows
         return _lib.lib.of_tc_splitk_plan(ctypes.byref(g))
-    if torch.cuda.is_available() and torch.cuda.get_device_properties(0).multi_processor_count != 148:
-        pytest.skip('the expected plans below are for 148 SMs')
-    assert plan(2048, 256, 256, 27) == 9          # 108 K blocks, 16 tiles: 9 ranges of 12 (144 CTAs)
-    assert plan(2048, 128, 512, 27) == 9          # 216 K blocks, 16 tiles
-    assert plan(2048, 128, 128, 27) == 9          # 54 K blocks: 9 ranges of 6
+    if torch.cuda.is_available() and torch.cuda.get_device_properties(0).multi_processor_count != 132:
+        pytest.skip('the expected plans below are for 132 SMs')
+    assert plan(2048, 256, 256, 27) == 6          # 108 K blocks, 16 tiles: 6 ranges of 18 (96 CTAs)
+    assert plan(2048, 128, 512, 27) == 8          # 216 K blocks, 16 tiles: 8 ranges of 27 (128 CTAs)
+    assert plan(2048, 128, 128, 27) == 6          # 54 K blocks: 6 ranges of 9
     assert plan(2048, 256, 256, 1) == 1           # 4 K blocks: nothing to split
     assert plan(16384, 128, 128, 27) == 1         # 128 tiles already fill the SMs
     assert plan(907484, 128, 128, 7, 5) == 1
     assert plan(2048, 250, 256, 27) == 1          # N must be a multiple of 32
-    assert plan(2048, 256, 100, 27) == 1          # c must be a multiple of 64 (tcgen05 path)
+    assert plan(2048, 256, 100, 27) == 1          # c must be a multiple of 64 (tensor-core path)
     assert _lib.lib.of_tc_splitk_plan(None) == 1
 
 
@@ -88,11 +88,14 @@ def test_hr_layout_matches_module_tree(cfg):
         assert 'unet_hr.' + p + key in shapes
 
 
-@pytest.mark.reference
 @pytest.mark.parametrize('cfg', [UNCOND, COND])
 def test_state_dict_parity_with_reference(cfg):
-    ref = ref_import.load()
-    want = {k: tuple(v.shape) for k, v in ref.union.UNet3DModel('hr', **cfg).state_dict().items()}
+    """state_dict shapes of the reference's UNet3DModel (tests/golden/state_shapes.json, oracle/gen_golden.py)"""
+    import json
+    from tests.util import GOLDEN
+    with open(os.path.join(GOLDEN, 'state_shapes.json')) as f:
+        table = json.load(f)
+    want = {k: tuple(v) for k, v in table['cond' if cfg is COND else 'uncond'].items()}
     assert want == model_shapes(cfg)
 
 

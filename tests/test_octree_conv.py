@@ -3,7 +3,7 @@ ocnn is third-party and absent: parity is UNPINNED at that boundary (SURVEY.md s
   * CPU: the oracle restatement equals torch conv3d (zero padding) on a full octree layer -- a known-answer check that
     does not depend on ocnn;
   * GPU: the CUDA path (of_octree_neigh27 + tap-gather GEMM) equals the oracle on full and adaptive layers, stride 1 / 2,
-    nempty, fp32 (CUDA cores) and bf16 (tcgen05)."""
+    nempty, fp32 (CUDA cores) and bf16 (tensor cores)."""
 import pytest
 import torch
 import torch.nn.functional as F

@@ -1,187 +1,121 @@
-"""Pins the oracle (oracle/restate.py) against the UNMODIFIED reference modules imported from
-/root/reference (build container only: skipped where the reference tree is absent)."""
+"""Pins the oracle (oracle/restate.py) against outputs of the UNMODIFIED reference modules, stored in
+tests/golden/reference_parity.npz by oracle/gen_golden.py (the reference itself is not needed to run these)."""
+import os
+import numpy as np
 import pytest
 import torch
 
-from oracle import restate as R, ref_import
-from tests.util import relerr, oracle_doctree, UNCOND, COND, SMALL
-
-pytestmark = pytest.mark.reference
+from oracle import restate as R
+from oracle.gen_golden import graph_digests, octree_digests, operator_inputs, split_signal, mpu_inputs, OPERATOR_GN_CHANNELS
+from tests.util import relerr, oracle_doctree, digest, GOLDEN
 
 
 @pytest.fixture(scope='module')
 def ref():
-    return ref_import.load()
-
-
-def _ref_doctree(ref, batch, seed):
-    from octfusion_b200.synth import synth_splits
-    from oracle.octree_util import octree_from_splits
-    l4, l5 = synth_splits(batch, seed)
-    doc = ref.dual_octree.DualOctree(octree_from_splits(l4, l5, batch))
-    doc.post_processing_for_docnn()
-    return doc
+    return np.load(os.path.join(GOLDEN, 'reference_parity.npz'))
 
 
 @pytest.mark.parametrize('batch,seed', [(1, 0), (2, 0), (3, 5)])
 def test_dual_graph_equals_reference(ref, batch, seed):
-    doc = _ref_doctree(ref, batch, seed)
     dg, _ = oracle_doctree(batch, seed)
-    for d in range(4, 7):
-        a, b = R.edge_set(doc.graph[d]), R.edge_set(dg.graph[d])
-        assert torch.equal(a[0], b[0]) and torch.equal(a[1], b[1])
-        assert torch.equal(doc.graph[d]['node_type'], dg.graph[d]['node_type'])
-        assert torch.equal(doc.batch_id(d), dg.batch_id(d))
-    assert torch.equal(doc.nnum, dg.nnum) and torch.equal(doc.lnum, dg.lnum)
+    pre = 'graph_b%d_s%d_' % (batch, seed)
+    for k, v in graph_digests(dg).items():
+        assert v == ref[pre + k], k
+    assert np.array_equal(dg.nnum.numpy(), ref[pre + 'nnum']) and np.array_equal(dg.lnum.numpy(), ref[pre + 'lnum'])
 
 
 @pytest.mark.parametrize('name', ['small', 'uncond', 'cond'])
 def test_full_unet_equals_reference(ref, name):
-    cfg = {'uncond': UNCOND, 'cond': COND, 'small': SMALL}[name]
-    net = ref.union.UNet3DModel('hr', **cfg).eval()
-    sd = R.seeded_state_dict({k: tuple(v.shape) for k, v in net.state_dict().items()}, 1)
-    net.load_state_dict(sd)
-    batch = 1 if name != 'small' else 2
-    doc = _ref_doctree(ref, batch, 0)
-    dg, _ = oracle_doctree(batch, 0)
-    g = torch.Generator().manual_seed(7)
-    x = torch.randn(doc.total_num, 3, generator=g)
-    ts = torch.tensor([1.5, -0.5])[:batch]
-    label = torch.tensor([1, 3])[:batch] if cfg.get('num_classes') else None
-    with torch.no_grad():
-        want = net(unet_type='hr', x=x, doctree=doc, timesteps=ts, unet_lr=net.unet_lr, label=label)
+    """full HR forward of the oracle against the reference's UNet3DModel.  Its own inputs (weights, latent, timesteps,
+    labels: oracle/gen_golden.py parity_unet_inputs), not those of the unet_<name>.npz fixtures."""
+    from oracle.gen_golden import PARITY_UNET, PARITY_UNET_ROW_STEP, parity_unet_inputs
+    from tests.util import model_shapes
+    dg, _ = oracle_doctree(PARITY_UNET[name], 0)
+    cfg, wseed, x, ts, label = parity_unet_inputs(name, dg.total_num)
     lr_cfg, hr_cfg = R.split_cfg(cfg)
-    got = R.hr_forward(x, dg, ts, sd, hr_cfg, lr_cfg, label=label)
-    assert float(want.abs().max()) > 0.1          # the seeded weights must not leave the net at zero
-    assert relerr(got, want) < 2e-5
+    got = R.hr_forward(x, dg, ts, R.seeded_state_dict(model_shapes(cfg), wseed), hr_cfg, lr_cfg, label=label)
+    assert float(ref['unet_%s_absmax' % name]) > 0.1          # the seeded weights must not leave the net at zero
+    assert relerr(got[::PARITY_UNET_ROW_STEP], torch.from_numpy(ref['unet_%s_y' % name])) < 2e-5
 
 
 def test_operators_equal_reference(ref):
-    m = ref.modules
-    doc = _ref_doctree(ref, 2, 0)
     dg, _ = oracle_doctree(2, 0)
-    g = torch.Generator().manual_seed(3)
+    inp = operator_inputs(dg, dg)
     # config-1 analogue: GraphConv 8->8 on the depth-4 full layer
-    conv = m.GraphConv(8, 8, 7, 7, 0)
-    x = torch.randn(2 * 4096, 8, generator=g)
-    with torch.no_grad():
-        assert relerr(R.graph_conv(x, dg.graph[4], conv.weights.data, 0), conv(x, doc, 4)) < 1e-6
-    conv = m.GraphConv(16, 24, 7, 7, 5)
-    x = torch.randn(dg.batch_id(6).shape[0], 16, generator=g)
-    with torch.no_grad():
-        assert relerr(R.graph_conv(x, dg.graph[6], conv.weights.data, 5), conv(x, doc, 6)) < 1e-6
-    for c in (24, 64, 384):
-        gn = m.DualOctreeGroupNorm(c)
-        gn.weights.data.normal_(1, 0.1, generator=g); gn.bias.data.normal_(0, 0.1, generator=g)
-        x = torch.randn(dg.batch_id(5).shape[0], c, generator=g) * 2 + 0.5
-        with torch.no_grad():
-            assert relerr(R.doctree_group_norm(x, dg.batch_id(5), 2, gn.weights.data, gn.bias.data), gn(x, doc, 5)) < 1e-5
-    qkv = torch.randn(8, 96, 64, generator=g)
-    assert relerr(R.qkv_attention(qkv), m.QKVAttention()(qkv)) < 1e-6
-    t = torch.tensor([9.2, -2.3, 0.1])
-    assert relerr(R.timestep_embedding(t, 128), ref.util.timestep_embedding(t, 128)) < 1e-6
-    assert abs(float(R.beta_linear_log_snr(torch.tensor(0.3))) - float(ref.util.beta_linear_log_snr(torch.tensor(0.3)))) < 1e-6
+    assert relerr(R.graph_conv(inp['conv8_x'], dg.graph[4], inp['conv8_w'], 0)[::4], torch.from_numpy(ref['conv8_y'])) < 1e-6
+    assert relerr(R.graph_conv(inp['conv16_x'], dg.graph[6], inp['conv16_w'], 5)[::32], torch.from_numpy(ref['conv16_y'])) < 1e-6
+    for c in OPERATOR_GN_CHANNELS:
+        gam, bet, x = inp['gn'][c]
+        assert relerr(R.doctree_group_norm(x, dg.batch_id(5), 2, gam, bet)[::256], torch.from_numpy(ref['gn%d_y' % c])) < 1e-5
+    assert relerr(R.qkv_attention(inp['qkv']), torch.from_numpy(ref['attn_y'])) < 1e-6
+    assert relerr(R.timestep_embedding(inp['t'], 128), torch.from_numpy(ref['temb_y'])) < 1e-6
+    assert abs(float(R.beta_linear_log_snr(torch.tensor(0.3))) - float(ref['log_snr_0.3'])) < 1e-6
 
 
 def test_vae_decode_equals_reference(ref):
-    """GraphVAE (SURVEY.md 8f rank 1): state_dict parity of the product class and decode_code(update_octree=True) of
-    the oracle against the reference on two shapes; the oracle grows its octree with the reference's labels."""
-    import importlib
+    """GraphVAE (SURVEY.md 8f rank 1): state_dict parity of the product class with the reference's, and
+    decode_code(update_octree=True) of the oracle against the reference on two shapes; the oracle grows its octree with
+    the reference's labels."""
+    import json
     from tests import util as U
-    gv = importlib.import_module('models.networks.dualoctree_networks.graph_vae')
-    net = gv.GraphVAE(**U.VAE).eval()
-    assert {k: tuple(v.shape) for k, v in net.state_dict().items()} == U.vae_shapes()
-    sd = U.vae_state_dict(5)
-    net.load_state_dict(sd)
-    doc = _ref_doctree(ref, 2, 3)
-    code = U.vae_code(doc.total_num, 2)
-    with torch.no_grad():
-        out = net.decode_code(code, doc, update_octree=True)
-    labels = {d: out['logits'][d].argmax(1) for d in (6, 7, 8)}
+    with open(os.path.join(GOLDEN, 'state_shapes.json')) as f:
+        assert {k: tuple(v) for k, v in json.load(f)['vae'].items()} == U.vae_shapes()
+    nnum = ref['vae_nnum']
+    labels = {d: torch.from_numpy(np.unpackbits(ref['vae_label%d' % d])[: int(nnum[d])].astype(np.int64)) for d in (6, 7, 8)}
     dg, _ = oracle_doctree(2, 3)
     mine = R.DualGraph(U.oracle_child_octree(dg.octree))
-    logits, regs, octree = R.vae_decode(code, mine, sd, 6, 8, 2, update_octree=True, labels=labels)
-    assert torch.equal(octree.nnum, out['octree_out'].nnum)
+    code = U.vae_code(dg.total_num, 2)
+    logits, regs, octree = R.vae_decode(code, mine, U.vae_state_dict(5), 6, 8, 2, update_octree=True, labels=labels)
+    assert np.array_equal(octree.nnum.numpy(), nnum)
+    for k, v in octree_digests(octree, (6, 7, 8)).items():
+        assert v == ref['vae_' + k], k
     for d in (6, 7, 8):
-        assert torch.equal(octree.keys[d], out['octree_out'].keys[d])
-        assert torch.equal(octree.children[d], out['octree_out'].children[d])
-        assert relerr(logits[d], out['logits'][d]) < 1e-5 and relerr(regs[d], out['reg_voxs'][d]) < 1e-5
+        assert relerr(logits[d][::32], torch.from_numpy(ref['vae_logit%d' % d])) < 1e-5
+        assert relerr(regs[d][::32], torch.from_numpy(ref['vae_reg%d' % d])) < 1e-5
 
 
 def test_vae_encode_equals_reference(ref):
     """GraphVAE.octree_encoder_step + KL_conv on given input features (the reference builds them from point clouds
-    with ocnn InputFeature, which is outside the path: `_get_input_feature` is replaced by a seeded tensor)."""
-    import importlib
-    import os
-    import numpy as np
+    with ocnn InputFeature, which is outside the path: `_get_input_feature` was replaced by a seeded tensor)."""
     from tests import util as U
-    gv = importlib.import_module('models.networks.dualoctree_networks.graph_vae')
-    net = gv.GraphVAE(**U.VAE).eval()
-    sd = U.vae_state_dict()
-    net.load_state_dict(sd)
-    g = np.load(os.path.join(U.GOLDEN, 'vae_decode.npz'))
+    g = np.load(os.path.join(GOLDEN, 'vae_decode.npz'))
     labels = {d: torch.from_numpy(np.unpackbits(g['label%d' % d])[: int(g['nnum'][d])].astype(np.int64)) for d in (6, 7, 8)}
     octree = U.oracle_grown_octree(labels)
-    doc = ref.dual_octree.DualOctree(octree)
-    doc.post_processing_for_docnn()
-    data = torch.randn(doc.total_num, 4, generator=torch.Generator().manual_seed(9))
-    net._get_input_feature = lambda doctree: data
-    with torch.no_grad():
-        convs = net.octree_encoder_step(octree, doc)
-        want = net.KL_conv(convs[6])
-    mine = R.vae_encode(data, R.DualGraph(octree), sd, 8, 6, 2)
-    assert relerr(mine, want) < 1e-5
+    dg = R.DualGraph(octree)
+    data = torch.randn(dg.total_num, 4, generator=torch.Generator().manual_seed(9))
+    mine = R.vae_encode(data, dg, U.vae_state_dict(), 8, 6, 2)
+    assert relerr(mine[::32], torch.from_numpy(ref['vae_encode_y'])) < 1e-5
 
 
-def test_split_octree_handoff_equals_reference():
+def test_split_octree_handoff_equals_reference(ref):
     """stage-1 -> stage-2 handoff (SURVEY.md 8f rank 2): split2octree_small / octree2split_small of the product
     (device-agnostic index ops) against the reference's, on a random split signal and its round trip."""
-    from oracle.ref_import import load_util
     from octfusion_b200 import octree as P
-    util = load_util()
-    g = torch.Generator().manual_seed(4)
-    split = torch.randn(2, 8, 16, 16, 16, generator=g)
-    split[torch.rand(split.shape, generator=g) < 0.6] = -1.0            # sparse, like a surface
-    want = util.split2octree_small(split.clone(), 6, 4)
-    got = P.split2octree_small(split, 6, 4)
-    assert got.depth == want.depth == 6
-    for d in range(4, 7):
-        assert torch.equal(got.keys[d], want.keys[d]) and torch.equal(got.children[d], want.children[d].int())
-    assert got.nnum.tolist() == want.nnum.tolist() and got.nnum_nempty.tolist() == want.nnum_nempty.tolist()
-    back_want = util.octree2split_small(want, 4)
+    got = P.split2octree_small(split_signal(), 6, 4)
+    assert got.depth == 6
+    for k, v in octree_digests(got, (4, 5, 6)).items():
+        assert v == ref['split_' + k], k
+    assert got.nnum.tolist() == ref['split_nnum'].tolist() and got.nnum_nempty.tolist() == ref['split_nnum_nempty'].tolist()
     back = P.octree2split_small(got, 4)
-    assert torch.equal(back, back_want)
+    assert digest(back.flatten().long()) == ref['split_back']
+    assert abs(float(back.double().abs().sum()) - float(ref['split_back_sum'])) < 1e-6
     # round trip: the octree built from its own split signal is the same octree
     again = P.split2octree_small(back, 6, 4)
     for d in range(4, 7):
         assert torch.equal(again.keys[d], got.keys[d]) and torch.equal(again.children[d], got.children[d])
 
 
-def test_neural_mpu_equals_reference(ref, monkeypatch):
-    """NeuralMPU (SURVEY.md 8f rank 4, oracle only): per-point restatement against reference mpu.py on the octree and
-    regression values of the VAE fixture case.  mpu.py:136 hard-codes `.cuda()`; on this CPU-only host it is patched
-    to the identity."""
-    import importlib
-    import os
-    import numpy as np
+def test_neural_mpu_equals_reference(ref):
+    """NeuralMPU (SURVEY.md 8f rank 4, oracle only): per-point restatement against reference mpu.py on the octree of the
+    VAE fixture case, query points near occupied depth-8 cells and uniform ones."""
     from tests import util as U
-    mpu = importlib.import_module('models.networks.dualoctree_networks.mpu')
-    monkeypatch.setattr(torch.Tensor, 'cuda', lambda self, *a, **k: self)
-    g = np.load(os.path.join(U.GOLDEN, 'vae_decode.npz'))
+    g = np.load(os.path.join(GOLDEN, 'vae_decode.npz'))
     labels = {d: torch.from_numpy(np.unpackbits(g['label%d' % d])[: int(g['nnum'][d])].astype(np.int64)) for d in (6, 7, 8)}
     octree = U.oracle_grown_octree(labels)
-    gen = torch.Generator().manual_seed(21)
-    ntot = {d: int(octree.nnum[4:d + 1].sum()) for d in (6, 7, 8)}
-    reg = {d: torch.randn(ntot[d], 4, generator=gen) for d in (6, 7, 8)}
-    # query points: near occupied depth-8 cells (so that every depth contributes) plus uniform ones (mostly coarse)
-    x, y, z, b = octree.xyzb(8)
-    pick = torch.randperm(x.numel(), generator=gen)[:4000]
-    near = (torch.stack([x, y, z], 1)[pick].float() + torch.rand(4000, 3, generator=gen)) / 128.0 - 1.0
-    uni = torch.rand(4000, 3, generator=gen) * 2 - 1
-    pos = torch.cat([torch.cat([near, uni]), torch.zeros(8000, 1)], 1)
-    want = mpu.NeuralMPU(4, 6, 8)(pos, reg, octree)
+    pos, reg = mpu_inputs(octree, 4000, 22)
     mine = R.mpu_eval(pos, reg, octree, 4, 6, 8)
     for d in (6, 7, 8):
-        assert torch.equal(mine[d][1], want[d][1])
-        assert relerr(mine[d][0], want[d][0]) < 1e-5, d
-    assert bool(want[8][1].any()) and not bool(want[8][1].all())
+        assert np.array_equal(np.packbits(mine[d][1].numpy()), ref['mpu_flag%d' % d])
+        assert relerr(mine[d][0], torch.from_numpy(ref['mpu_fval%d' % d])) < 1e-5, d
+    flag8 = np.unpackbits(ref['mpu_flag8'])[: mine[8][1].numel()]
+    assert flag8.any() and not flag8.all()

@@ -62,6 +62,15 @@ def build_product(cfg, sd, device='cuda', stage='hr'):
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), 'golden')
 
 
+def digest(a) -> str:
+    """sha256 of an integer array as little-endian int64: exact comparison of large integer results (graphs, octrees)
+    against a fixture of a few bytes"""
+    import hashlib
+    import numpy as np
+    a = a.cpu().numpy() if torch.is_tensor(a) else np.asarray(a)
+    return hashlib.sha256(np.ascontiguousarray(a.astype('<i8')).tobytes()).hexdigest()
+
+
 # ---- GraphVAE decoder (SURVEY.md 8f rank 1; reference configs/vae_snet_train.yaml) ----
 VAE = dict(depth=8, channel_in=4, nout=4, full_depth=4, depth_stop=6, depth_out=8, resblk_type='basic', bottleneck=4,
            resblk_num=2, code_channel=16, embed_dim=3)

@@ -1,4 +1,4 @@
-"""Single-kernel driver for ncu: one GraphConv (tcgen05 tap-gather GEMM) at the full B=32 size.
+"""One GraphConv (tensor-core tap-gather GEMM) at the full B=32 size, timed with CUDA events.
 usage: python tools/prof_conv.py [depth cin cout] ; env REPS"""
 import os, sys, time
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
