@@ -9,15 +9,20 @@
 // The im2col buffer is never written to HBM: producer warps build each [128 x 64] bf16 A tile
 // directly in shared memory, in the 128-byte-swizzled K-major layout wgmma reads.
 //
-// One persistent CTA per SM, 384 threads = three warpgroups:
+// One persistent CTA per SM, launched as clusters of two for BN >= 128 (TcCfg::CLUSTER): the CTAs of a pair compute two
+// adjacent 128-row tiles of the same columns and K range, so they need the same weight tiles, and each fetches half of
+// every weight tile for both.
+// 384 threads = three warpgroups:
 //   warpgroup 0    producers: each warp fills every PW-th stage of the shared-memory ring (PW = 4, or the ring depth
 //                  when it is shallower).  Tap table -> thirty-two 16-byte cp.async (LDGSTS) per lane straight into the
 //                  swizzled A stage, completion by cp.async.mbarrier.arrive.noinc; lane 0 also streams the stage's
-//                  pre-swizzled [BN x 64] weight tile with cp.async.bulk (1-D TMA) onto the same full barrier.  The
-//                  table entries of the warp's next stage are fetched before it waits for the current one to be freed.
+//                  pre-swizzled [BN x 64] weight tile with cp.async.bulk (1-D TMA) onto the same full barrier -- in a
+//                  pair, its half with .multicast::cluster into the slot of both CTAs.  The table entries of the warp's next stage are
+//                  fetched before it waits for the current one to be freed (by the consumers of both CTAs).
 //   warpgroups 1-2 consumers, 64 rows of the 128-row tile each: wgmma 64 x BN x 16 from shared memory into register
 //                  accumulators, one stage in flight; then the epilogue: accumulators -> shared-memory staging (64
-//                  columns at a time) -> +bias/+emb[batch]/+residual, store; optionally the group-norm partial statistics
+//                  columns at a time; BN = 256 stages through the ring slot of the tile's last K block)
+//                  -> +bias/+emb[batch]/+residual, store; optionally the group-norm partial statistics
 //                  of the tile (warp-shuffle reduction, one write per 32-row chunk -- no atomics, bit-reproducible): the
 //                  statistics pass of the following DualOctreeGroupNorm (modules.py:291-326) never reads the tensor again.
 // While the consumers drain a tile the producers already fill the ring with the next tile's stages.
@@ -56,25 +61,67 @@ __device__ __forceinline__ void mbar_arrive(uint32_t bar) {
 __device__ __forceinline__ void mbar_arrive_expect_tx(uint32_t bar, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
 }
+// CLUSTER: acquire at cluster scope (the barrier also counts arrivals of the peer CTA's threads)
+template <bool CLUSTER>
 __device__ __forceinline__ bool mbar_try_wait(uint32_t bar, uint32_t parity) {
   uint32_t ok;
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-      "selp.u32 %0, 1, 0, p;\n\t}"
-      : "=r"(ok)
-      : "r"(bar), "r"(parity)
-      : "memory");
+  if constexpr (CLUSTER)
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "mbarrier.try_wait.parity.acquire.cluster.shared::cta.b64 p, [%1], %2;\n\t"
+        "selp.u32 %0, 1, 0, p;\n\t}"
+        : "=r"(ok)
+        : "r"(bar), "r"(parity)
+        : "memory");
+  else
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
+        "selp.u32 %0, 1, 0, p;\n\t}"
+        : "=r"(ok)
+        : "r"(bar), "r"(parity)
+        : "memory");
   return ok != 0;
 }
 // Bounded wait: a protocol bug becomes a trap (an error the host sees), never a hung GPU.  (No printf here: a function
 // call inside the consumers' MMA loop would make ptxas serialise the wgmma pipeline.)
+template <bool CLUSTER = false>
 __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
-  if (mbar_try_wait(bar, parity)) return;
+  if (mbar_try_wait<CLUSTER>(bar, parity)) return;
   const long long t0 = clock64();
-  while (!mbar_try_wait(bar, parity)) {
+  while (!mbar_try_wait<CLUSTER>(bar, parity)) {
     if (clock64() - t0 > 4000000000ll) __trap();
   }
+}
+// ---- CTA pairs (thread-block clusters of 2) ----
+__device__ __forceinline__ uint32_t cluster_ctarank() {
+  uint32_t r;
+  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
+  return r;
+}
+__device__ __forceinline__ uint32_t cluster_id_x() {
+  uint32_t r;
+  asm volatile("mov.u32 %0, %%clusterid.x;" : "=r"(r));
+  return r;
+}
+__device__ __forceinline__ uint32_t cluster_count_x() {
+  uint32_t r;
+  asm volatile("mov.u32 %0, %%nclusterid.x;" : "=r"(r));
+  return r;
+}
+// every thread of both CTAs; orders the mbarrier inits before any remote arrive or multicast, and keeps a CTA resident
+// until its peer can no longer write into its shared memory
+__device__ __forceinline__ void cluster_sync() {
+  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
+}
+// the address of the same shared-memory location in CTA `rank` of the cluster
+__device__ __forceinline__ uint32_t mapa_shared(uint32_t addr, uint32_t rank) {
+  uint32_t r;
+  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(addr), "r"(rank));
+  return r;
+}
+__device__ __forceinline__ void mbar_arrive_remote(uint32_t cluster_bar) {
+  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_bar) : "memory");
 }
 // register budget of a warpgroup (the producers give theirs to the accumulators of the consumers)
 template <int R> __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
@@ -86,6 +133,12 @@ __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.p
 __device__ __forceinline__ void bulk_g2s(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar) {
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst),
                "l"(src), "r"(bytes), "r"(bar)
+               : "memory");
+}
+// the same bytes into the same CTA-relative address of every CTA in `mask`, each completing its own copy of `bar`
+__device__ __forceinline__ void bulk_g2s_multicast(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar, uint16_t mask) {
+  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1], %2, [%3], %4;"
+               ::"r"(dst), "l"(src), "r"(bytes), "r"(bar), "h"(mask)
                : "memory");
 }
 __device__ __forceinline__ void named_bar_sync(int id, int threads) {
@@ -175,6 +228,10 @@ template <> struct Wgmma<256> {
 // ------------------------------------------------------------------------------------------------
 // BN: output columns per tile (the wgmma N).  A stage holds one 64-wide K block of the 128-row A tile and of the weight
 // tile; the ring takes what is left of the 227 KB beside the epilogue staging and the barriers.
+// EPI_IN_RING (BN = 256): the 34 KB staging fits in one 48 KB stage, so the consumers stage the epilogue through the
+// ring slot of the tile's last K block and release it only after the epilogue; the ring is then 4 deep instead of 3.
+// The narrower tiles keep a dedicated staging buffer and their ring depths (5 for 128, 7 for 64, 9 for 32, 11 for 16):
+// a 6-deep BN = 128 ring (staging rows XOR-swizzled to fit its 32 KB slot) measured no faster.
 template <int BN>
 struct TcCfg {
   static constexpr int A_BYTES = TC_BM * 128;
@@ -183,14 +240,22 @@ struct TcCfg {
   static constexpr int EPI_COLS = BN < 64 ? BN : 64;                // columns per epilogue round
   static constexpr int EPI_LD = EPI_COLS + 4;                       // staging row stride in floats (conflict-free float4 rows)
   static constexpr int EPI_BYTES = 2 * 64 * EPI_LD * 4;             // one 64-row block per consumer warpgroup
+  static constexpr bool EPI_IN_RING = BN == 256;
+  // CTAs per cluster: pairs share the weight tiles of BN >= 128 (16-32 KB per stage, as much as or more than the A tile).
+  // The narrower weight tiles are 2-8 KB; there sharing saves little and the lockstep of the pair cost the narrow
+  // (VAE) layers more than it saved, so those launch single CTAs, each fetching its whole weight tile.
+  static constexpr int CLUSTER = BN >= 128 ? 2 : 1;
+  static constexpr int EPI_OWN_BYTES = EPI_IN_RING ? 0 : EPI_BYTES; // staging outside the ring
   static constexpr int AUX_BYTES = 1024 + 8 * 1024;                 // mbarriers | per-consumer-warp row of (bias + emb)
-  static constexpr int FIT = (TC_SMEM_MAX - 1024 - EPI_BYTES - AUX_BYTES) / STAGE_BYTES;
+  static constexpr int FIT = (TC_SMEM_MAX - 1024 - EPI_OWN_BYTES - AUX_BYTES) / STAGE_BYTES;
   static constexpr int STAGES = FIT > 16 ? 16 : FIT;
   // producer warps.  A warp that waits for the release of its slot must know that the slot's previous use has been
   // released as well (the mbarrier parity tells two phases apart, not three): PW <= STAGES guarantees it.
   static constexpr int PW = STAGES < 4 ? STAGES : 4;
-  static constexpr int SMEM_BYTES = 1024 /*align slack*/ + STAGES * STAGE_BYTES + EPI_BYTES + AUX_BYTES;
+  static constexpr int SMEM_BYTES = 1024 /*align slack*/ + STAGES * STAGE_BYTES + EPI_OWN_BYTES + AUX_BYTES;
   static_assert(STAGES >= 2 && SMEM_BYTES <= TC_SMEM_MAX, "ring depth");
+  static_assert(!EPI_IN_RING || EPI_BYTES <= STAGE_BYTES, "staging must fit one ring slot");
+  static_assert(B_BYTES % 32 == 0, "each CTA of a pair copies one 16-byte-aligned half of the weight tile");
 };
 
 struct TcParams {
@@ -207,19 +272,22 @@ struct TcParams {
 // afterwards a[0] of lane L holds the warp total of the ORIGINAL a[(L >> 1) & 15]; NV = 32: 16+8+4+2+1 = 31 shuffles,
 // a[0] of lane L holds the total of the original a[L] (a plain butterfly needs 5 * NV).  The order of the additions
 // is fixed, so the result is bit-reproducible.
-template <int NV>
+// One halving level per instantiation: with the level a compile-time constant every a[] index is one, and the array
+// stays in registers (a runtime level loop left the multi-segment path indexing a[] in local memory).
+template <int NV, int HALF = NV / 2, int BIT = 16>
 __device__ __forceinline__ void warp_reduce_vals(float (&a)[NV], int lane) {
+  if constexpr (HALF >= 1) {
+    const bool up = (lane & BIT) != 0;
 #pragma unroll
-  for (int half = NV / 2, bit = 16; half >= 1; half >>= 1, bit >>= 1) {
-    const bool up = (lane & bit) != 0;
-#pragma unroll
-    for (int i = 0; i < half; ++i) {
-      const float send = up ? a[i] : a[i + half];
-      const float keep = up ? a[i + half] : a[i];
-      a[i] = keep + __shfl_xor_sync(0xffffffffu, send, bit);
+    for (int i = 0; i < HALF; ++i) {
+      const float send = up ? a[i] : a[i + HALF];
+      const float keep = up ? a[i + HALF] : a[i];
+      a[i] = keep + __shfl_xor_sync(0xffffffffu, send, BIT);
     }
+    warp_reduce_vals<NV, HALF / 2, BIT / 2>(a, lane);
+  } else if constexpr (NV == 16) {
+    a[0] += __shfl_xor_sync(0xffffffffu, a[0], 1);
   }
-  if (NV == 16) a[0] += __shfl_xor_sync(0xffffffffu, a[0], 1);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -230,8 +298,8 @@ __global__ void __launch_bounds__(TC_THREADS, 1) gather_gemm_tc_kernel(const __g
   using Cfg = TcCfg<BN>;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const uint32_t epi = smem_base + Cfg::STAGES * Cfg::STAGE_BYTES;
-  const uint32_t aux = epi + Cfg::EPI_BYTES;
+  const uint32_t epi = smem_base + Cfg::STAGES * Cfg::STAGE_BYTES;   // (dedicated staging, when not EPI_IN_RING)
+  const uint32_t aux = epi + Cfg::EPI_OWN_BYTES;
   const uint32_t bar_full = aux, bar_empty = aux + 128;             // one pair per ring slot
 
   const int wg = threadIdx.x >> 7, t = threadIdx.x & 127;
@@ -239,16 +307,23 @@ __global__ void __launch_bounds__(TC_THREADS, 1) gather_gemm_tc_kernel(const __g
   const of_gemm_args& g = p.g;
   const int taps = g.taps;
   const int ksplit = p.ksplit;
-  const int total_tiles = p.m_tiles * p.n_tiles * ksplit;   // virtual tile v: output tile v / ksplit, K range v % ksplit
+  // CTA pairs (Cfg::CLUSTER = 2): a work unit is (two adjacent 128-row M tiles, N tile, K range); CTA `rank` of the
+  // cluster takes M tile 2 * pair + rank, both walk the same units and K blocks, and each copies one half of the shared
+  // weight tile into both.  With single CTAs a unit is one M tile.  Virtual unit v: output unit v / ksplit, K range
+  // v % ksplit.
+  constexpr int CL = Cfg::CLUSTER;
+  const int rank = CL == 2 ? (int)cluster_ctarank() : 0;
+  const int cid = (int)cluster_id_x(), nclusters = (int)cluster_count_x();
+  const int total_units = (p.m_tiles + CL - 1) / CL * p.n_tiles * ksplit;
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < Cfg::STAGES; ++s) {
       mbar_init(bar_full + 8 * s, 32 + 1);                  // the producer warp's lanes + the weight copy's expect_tx
-      mbar_init(bar_empty + 8 * s, 2);                      // the two consumer warpgroups
+      mbar_init(bar_empty + 8 * s, 2 * CL);                 // the two consumer warpgroups of each CTA of the cluster
     }
     fence_mbar_init();
   }
-  __syncthreads();
+  cluster_sync();
 
   if (wg == 0) {
     // =========================== producers ===========================
@@ -260,16 +335,17 @@ __global__ void __launch_bounds__(TC_THREADS, 1) gather_gemm_tc_kernel(const __g
       const __nv_bfloat16* a1 = reinterpret_cast<const __nv_bfloat16*>(g.a1);
       const int32_t* __restrict__ tab = g.tap_tab;
       const uint8_t* wp = reinterpret_cast<const uint8_t*>(g.w);
-      const int my_tiles = (total_tiles - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;
-      const int total_stages = my_tiles * p.num_kb;
+      const int my_units = (total_units - cid + nclusters - 1) / nclusters;
+      const int total_stages = my_units * p.num_kb;
       struct Pos { int m0, n0, kabs; };
-      // stage s of this CTA -> rows, columns and ABSOLUTE K block (split-K: the K range's offset included)
+      // stage s of this CTA -> rows, columns and ABSOLUTE K block (split-K: the K range's offset included); the rows
+      // of the second CTA of the last pair lie beyond M when the number of M tiles is odd
       auto pos_of = [&](int s) {
-        const int ti = s / p.num_kb, kb = s - ti * p.num_kb;
-        const int tile = (int)blockIdx.x + ti * (int)gridDim.x;
-        const int vtile = g.reverse ? total_tiles - 1 - tile : tile;
-        const int ptile = vtile / ksplit;
-        return Pos{(ptile / p.n_tiles) * TC_BM, (ptile % p.n_tiles) * BN, (vtile - ptile * ksplit) * p.num_kb + kb};
+        const int ui = s / p.num_kb, kb = s - ui * p.num_kb;
+        const int unit = cid + ui * nclusters;
+        const int vunit = g.reverse ? total_units - 1 - unit : unit;
+        const int ptile = vunit / ksplit;
+        return Pos{((ptile / p.n_tiles) * CL + rank) * TC_BM, (ptile % p.n_tiles) * BN, (vunit - ptile * ksplit) * p.num_kb + kb};
       };
       auto fetch_taps = [&](const Pos& c, int32_t (&tv)[32]) {
         const int cb = c.kabs / taps;
@@ -296,12 +372,17 @@ __global__ void __launch_bounds__(TC_THREADS, 1) gather_gemm_tc_kernel(const __g
         if (s + Cfg::PW < total_stages) fetch_taps(pos_of(s + Cfg::PW), tnext);
         const int stage = s % Cfg::STAGES;
         const uint32_t phase = (uint32_t)(s / Cfg::STAGES) & 1u;
-        mbar_wait(bar_empty + 8 * stage, phase ^ 1);
+        // released by the consumers of both CTAs: the peer's producer writes its half of the weight tile into this slot
+        mbar_wait<true>(bar_empty + 8 * stage, phase ^ 1);
         const uint32_t a_addr = smem_base + stage * Cfg::STAGE_BYTES;
         const uint32_t full = bar_full + 8 * stage;
         if (lane == 0) {
+          // the whole tile lands here; in a pair, this CTA's half and the peer's, each multicast to both CTAs
+          constexpr uint32_t PART = Cfg::B_BYTES / CL;
+          const uint8_t* src = wp + ((int64_t)c.kabs * p.npad + c.n0) * 128 + rank * PART;
           mbar_arrive_expect_tx(full, (uint32_t)Cfg::B_BYTES);
-          bulk_g2s(a_addr + Cfg::A_BYTES, wp + ((int64_t)c.kabs * p.npad + c.n0) * 128, Cfg::B_BYTES, full);
+          if constexpr (CL == 2) bulk_g2s_multicast(a_addr + Cfg::A_BYTES + rank * PART, src, PART, full, (uint16_t)0x3);
+          else bulk_g2s(a_addr + Cfg::A_BYTES, src, PART, full);
         }
         const int cb = c.kabs / taps;
         if (cb < p.cblocks) {
@@ -358,11 +439,17 @@ __global__ void __launch_bounds__(TC_THREADS, 1) gather_gemm_tc_kernel(const __g
     float acc[BN / 2];
     int stage = 0;
     uint32_t phase = 0;
-    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-      const int vtile = g.reverse ? total_tiles - 1 - tile : tile;
-      const int ptile = vtile / ksplit;
-      const int64_t split_row0 = (int64_t)(vtile - ptile * ksplit) * g.M;        // this K range's slab of the workspace
-      const int m0 = (ptile / p.n_tiles) * TC_BM, n0 = (ptile % p.n_tiles) * BN;
+    const uint32_t peer_empty = CL == 2 ? mapa_shared(bar_empty, (uint32_t)rank ^ 1u) : 0u;
+    // a slot is free again once both consumer warpgroups of every CTA of the cluster are done with it
+    auto release = [&](int s) {
+      mbar_arrive(bar_empty + 8 * s);
+      if constexpr (CL == 2) mbar_arrive_remote(peer_empty + 8 * s);
+    };
+    for (int unit = cid; unit < total_units; unit += nclusters) {
+      const int vunit = g.reverse ? total_units - 1 - unit : unit;
+      const int ptile = vunit / ksplit;
+      const int64_t split_row0 = (int64_t)(vunit - ptile * ksplit) * g.M;        // this K range's slab of the workspace
+      const int m0 = ((ptile / p.n_tiles) * CL + rank) * TC_BM, n0 = (ptile % p.n_tiles) * BN;
 #pragma unroll
       for (int i = 0; i < BN / 2; ++i) fence_operand(acc[i]);
       int prev = 0;
@@ -376,14 +463,22 @@ __global__ void __launch_bounds__(TC_THREADS, 1) gather_gemm_tc_kernel(const __g
         for (int k = 0; k < TC_BK / 16; ++k) Wgmma<BN>::mma(acc, da + 2 * k, db + 2 * k, (kb > 0 || k > 0) ? 1u : 0u);
         wgmma_commit();
         wgmma_wait<1>();                                   // the previous stage's MMAs have read their operands
-        if (kb > 0 && t == 0) mbar_arrive(bar_empty + 8 * prev);
+        if (kb > 0 && t == 0) release(prev);
         prev = stage;
         if (++stage == Cfg::STAGES) { stage = 0; phase ^= 1u; }
       }
       wgmma_wait<0>();
 #pragma unroll
       for (int i = 0; i < BN / 2; ++i) fence_operand(acc[i]);
-      if (t == 0) mbar_arrive(bar_empty + 8 * prev);
+      uint32_t stg_base = epi;
+      if constexpr (Cfg::EPI_IN_RING) {
+        // the last K block's slot becomes the staging: both warpgroups' MMAs must have read all of it (the other
+        // warpgroup's A rows and the shared weight tile lie under this warpgroup's staging rows)
+        named_bar_sync(3, 256);
+        stg_base = smem_base + prev * Cfg::STAGE_BYTES;
+      } else {
+        if (t == 0) release(prev);
+      }
 
       // ---- epilogue: warp (w & 1) owns rows 32 (w & 1) .. +31 of the warpgroup's 64, column half (w >> 1) of each
       // staged 64-column block; lane = row ----
@@ -391,7 +486,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) gather_gemm_tc_kernel(const __g
       const int rl = (warp & 1) * 32 + lane;
       const int cc = (warp >> 1) * 32;
       const bool active = cc < Cfg::EPI_COLS;             // (warp-uniform)
-      const uint32_t stg = epi + (uint32_t)cw * 64 * Cfg::EPI_LD * 4;
+      const uint32_t stg = stg_base + (uint32_t)cw * 64 * Cfg::EPI_LD * 4;
       const int m = m0 + cw * 64 + rl;
       const bool row_ok = m < g.M;
       const int64_t orow = row_ok ? (g.out_rows ? (int64_t)g.out_rows[m] : (int64_t)m + split_row0) : 0;
@@ -574,9 +669,15 @@ __global__ void __launch_bounds__(TC_THREADS, 1) gather_gemm_tc_kernel(const __g
           process(v, blk * Cfg::EPI_COLS + cc);
         }
       }
+      if constexpr (Cfg::EPI_IN_RING) {
+        // the staging reads and writes (generic proxy) come before the next copies into the slot (async proxy)
+        fence_proxy_async_smem();
+        named_bar_sync(1 + cw, 128);
+        if (t == 0) release(prev);
+      }
     }
   }
-  __syncthreads();                                         // no CTA exits while its copies are in flight
+  cluster_sync();                                          // no CTA exits while its or its peer's copies are in flight
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -612,23 +713,47 @@ __global__ void pack_weight_tc_kernel(const float* __restrict__ w, int taps, int
 template <int BN>
 static int launch_tc(TcParams& p, cudaStream_t st) {
   using Cfg = TcCfg<BN>;
-  // the opt-in to > 48 KB of dynamic shared memory is a per-device attribute of the function
-  static bool configured[64] = {};
+  cudaLaunchAttribute cluster;
+  cluster.id = cudaLaunchAttributeClusterDimension;
+  cluster.val.clusterDim.x = Cfg::CLUSTER;
+  cluster.val.clusterDim.y = 1;
+  cluster.val.clusterDim.z = 1;
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3(Cfg::CLUSTER);
+  cfg.blockDim = dim3(TC_THREADS);
+  cfg.dynamicSmemBytes = Cfg::SMEM_BYTES;
+  cfg.stream = st;
+  cfg.attrs = &cluster;
+  cfg.numAttrs = 1;
+  // per device: the opt-in to > 48 KB of dynamic shared memory (an attribute of the function) and the number of
+  // clusters that can be resident at once (a pair is placed within a GPC, so not necessarily half the SM count)
+  static int max_clusters[64] = {};
   int dev = 0;
   cudaGetDevice(&dev);
-  if (dev < 0 || dev >= 64 || !configured[dev]) {
+  int clusters = (dev >= 0 && dev < 64) ? max_clusters[dev] : 0;
+  if (clusters == 0) {
     cudaError_t e = cudaFuncSetAttribute(gather_gemm_tc_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES);
     if (e != cudaSuccess) {
       set_error("of_gather_gemm_tc: cudaFuncSetAttribute(%d B): %s", Cfg::SMEM_BYTES, cudaGetErrorString(e));
       return OF_E_CUDA;
     }
-    if (dev >= 0 && dev < 64) configured[dev] = true;
+    e = cudaOccupancyMaxActiveClusters(&clusters, gather_gemm_tc_kernel<BN>, &cfg);
+    if (e != cudaSuccess || clusters < 1) {
+      set_error("of_gather_gemm_tc: no cluster of %d CTAs with %d B shared memory fits (%s)", Cfg::CLUSTER, Cfg::SMEM_BYTES,
+                e != cudaSuccess ? cudaGetErrorString(e) : "0 active clusters");
+      return OF_E_CUDA;
+    }
+    if (dev >= 0 && dev < 64) max_clusters[dev] = clusters;
   }
   p.m_tiles = (p.g.M + TC_BM - 1) / TC_BM;
   p.n_tiles = p.npad / BN;
-  const int total = p.m_tiles * p.n_tiles * p.ksplit;
-  const int grid = total < num_sms() ? total : num_sms();
-  gather_gemm_tc_kernel<BN><<<grid, TC_THREADS, Cfg::SMEM_BYTES, st>>>(p);
+  const int units = (p.m_tiles + Cfg::CLUSTER - 1) / Cfg::CLUSTER * p.n_tiles * p.ksplit;
+  cfg.gridDim = dim3(Cfg::CLUSTER * (units < clusters ? units : clusters));
+  const cudaError_t e = cudaLaunchKernelEx(&cfg, gather_gemm_tc_kernel<BN>, p);
+  if (e != cudaSuccess) {
+    set_error("of_gather_gemm_tc: launch failed: %s", cudaGetErrorString(e));
+    return OF_E_CUDA;
+  }
   OF_LAUNCH_CHECK("of_gather_gemm_tc");
   return OF_OK;
 }
