@@ -333,6 +333,34 @@ int of_mpu_eval(const of_octree_levels* oct, int32_t depth, const float* pos, in
 int of_mpu_eval_grid(const of_octree_levels* oct, int32_t depth, int32_t batch_idx, int32_t size, float bbmin,
                      float bbmax, int64_t head, int64_t count, const float* reg, float* fval, void* stream);
 
+/* ------------------------------------------------------------------------------------------
+ * Point-cloud shape metrics (reference metrics/evaluation_metrics.py: MMD, COV and 1-NNA with Chamfer distance and
+ * approximate EMD).  Clouds are contiguous fp32 [count, points, 3].  "All pairs" entries compute every (i, j) of
+ * a [na] x b [nb] into row-major [na, nb] outputs without copying any cloud; an entry is bit-identical to the same
+ * pair computed in paired mode, and every result is identical from run to run (no float atomics, fixed sum order).
+ * ------------------------------------------------------------------------------------------ */
+#define OF_EMD_MAX_POINTS 4096            /* largest n of of_match_cost / of_emd_cd_pairwise                  */
+#define OF_CD_PAIRWISE_MAX_POINTS 49152   /* largest P + Q of of_chamfer_pairwise                              */
+/* nndistance (metrics/pytorch_structural_losses/src/nndistance.cu:125-128) for `batch` pairs (a[i], b[i]):
+ * dist1 [batch, P]: dist1[i, k] = min_l |b_il - a_ik|^2, dist2 [batch, Q]: dist2[i, l] = min_k |b_il - a_ik|^2, with
+ * the reference's fp32 expression (bit-identical values); cd [batch] = mean(dist1[i]) + mean(dist2[i]), may be NULL.
+ * Any P, Q >= 1. */
+int of_nn_distance(const float* a, const float* b, int32_t batch, int32_t P, int32_t Q, float* dist1, float* dist2,
+                   float* cd, void* stream);
+/* all-pairs Chamfer distance of _pairwise_EMD_CD_ (metrics/evaluation_metrics.py:111-154, CD arm :133-137):
+ * cd [na, nb] = mean_k dist1 + mean_l dist2 of the pair (a_i, b_j).  P + Q <= OF_CD_PAIRWISE_MAX_POINTS. */
+int of_chamfer_pairwise(const float* a, int32_t na, int32_t P, const float* b, int32_t nb, int32_t Q, float* cd,
+                        void* stream);
+/* approxmatch + matchcost (metrics/pytorch_structural_losses/src/approxmatch.cu:299-316) for `batch` pairs
+ * (xyz1 = a[i], xyz2 = b[i]) of n points each: cost [batch] = sum_kl match_kl |b_l - a_k|, the reference's
+ * un-normalised cost (9 levels -4^7 .. -4^-1), without a match matrix.  cd [batch] (may be NULL) = the Chamfer
+ * distance of the same pair, as of_nn_distance computes it up to summation order.  1 <= n <= OF_EMD_MAX_POINTS. */
+int of_match_cost(const float* a, const float* b, int32_t batch, int32_t n, float* cost, float* cd, void* stream);
+/* all pairs of _pairwise_EMD_CD_ (metrics/evaluation_metrics.py:111-154) in one launch: cost [na, nb] as
+ * of_match_cost (emd = cost / n) and cd [na, nb] as of_match_cost's cd, for xyz1 = a_i, xyz2 = b_j. */
+int of_emd_cd_pairwise(const float* a, int32_t na, const float* b, int32_t nb, int32_t n, float* cost, float* cd,
+                       void* stream);
+
 #ifdef __cplusplus
 }
 #endif

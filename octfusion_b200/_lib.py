@@ -97,7 +97,14 @@ _PROTOS = {
     'of_octree_neigh27': (C.c_int, [C.POINTER(OctreeLevels), _i32, _vp, _vp]),
     'of_mpu_eval': (C.c_int, [C.POINTER(OctreeLevels), _i32, _vp, _i64, _vp, _vp, _vp, _vp]),
     'of_mpu_eval_grid': (C.c_int, [C.POINTER(OctreeLevels), _i32, _i32, _i32, _f32, _f32, _i64, _i64, _vp, _vp, _vp]),
+    'of_nn_distance': (C.c_int, [_vp, _vp, _i32, _i32, _i32, _vp, _vp, _vp, _vp]),
+    'of_chamfer_pairwise': (C.c_int, [_vp, _i32, _i32, _vp, _i32, _i32, _vp, _vp]),
+    'of_match_cost': (C.c_int, [_vp, _vp, _i32, _i32, _vp, _vp, _vp]),
+    'of_emd_cd_pairwise': (C.c_int, [_vp, _i32, _vp, _i32, _i32, _vp, _vp, _vp]),
 }
+
+EMD_MAX_POINTS = 4096              # OF_EMD_MAX_POINTS
+CD_PAIRWISE_MAX_POINTS = 49152     # OF_CD_PAIRWISE_MAX_POINTS
 
 EXPORTED_SYMBOLS = tuple(_PROTOS)
 

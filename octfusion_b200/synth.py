@@ -70,3 +70,15 @@ def slice_splits(label_fd, label_fd1, lo: int, hi: int, full_depth: int = 4):
     per = label_fd.view(-1, nfull).sum(1) * 8                  # depth-(fd+1) nodes per shape
     off = torch.cat([torch.zeros(1, dtype=per.dtype), torch.cumsum(per, 0)])
     return label_fd[lo * nfull: hi * nfull], label_fd1[int(off[lo]): int(off[hi])]
+
+
+def synth_point_clouds(n: int, points: int, seed: int) -> torch.Tensor:
+    """[n, points, 3] fp32 surface-like point clouds (the input of the shape metrics): per cloud, points on a random
+    ellipsoid shell (semi-axes 0.2 .. 0.45, random centre inside the unit cube) with 1 % radial noise."""
+    g = torch.Generator().manual_seed(seed)
+    direction = torch.randn(n, points, 3, generator=g)
+    direction = direction / direction.norm(dim=-1, keepdim=True)
+    axes = 0.2 + 0.25 * torch.rand(n, 1, 3, generator=g)
+    centre = 0.45 + 0.1 * torch.rand(n, 1, 3, generator=g)
+    radial = 1.0 + 0.01 * torch.randn(n, points, 1, generator=g)
+    return (centre + direction * axes * radial).float().contiguous()
