@@ -361,6 +361,41 @@ int of_match_cost(const float* a, const float* b, int32_t batch, int32_t n, floa
 int of_emd_cd_pairwise(const float* a, int32_t na, const float* b, int32_t nb, int32_t n, float* cost, float* cd,
                        void* stream);
 
+/* ------------------------------------------------------------------------------------------
+ * Meshes and metric point clouds.  Marching cubes replaces skimage.measure.marching_cubes(sdf, level) of export_mesh
+ * (models/octfusion_model_union.py:452-455); surface sampling replaces trimesh mesh.sample(count) and the bounding box
+ * feeds scale_to_unit_cube (metrics/generate_pointclouds.py:14-37).
+ *
+ * Grid: one [size, size, size] fp32 array of calc_sdf, sdf[i, j, k], i (x) slowest.  A corner is inside when
+ * f < level (f == level and NaN are outside).  Grid point p owns its edges p -> p + e_axis inside the grid; a crossing
+ * edge (one end inside) has one vertex at the lower-index end a plus t = (level - f_a) / (f_b - f_a) along the axis,
+ * in fp32 with correctly rounded sub, div and add, in index space.  Vertex ids run in (point linear index, axis)
+ * order; faces are int32 vertex-id triples in (cell linear index, table order), the table being generated by
+ * octfusion_b200/mc_table.py.  Faces wind so that (v1 - v0) x (v2 - v0) points from inside to outside.  The output
+ * is bit-reproducible and does not depend on the launch configuration.
+ * ------------------------------------------------------------------------------------------ */
+#define OF_MC_MAX_SIZE 512                /* largest grid side of of_mc_count / of_mc_emit                      */
+/* pass 1: vert_count[p] = crossing edges point p owns (0..3), tri_count[p] = triangles of the cell whose lowest corner
+ * is p (0..5; 0 on the far faces of the grid).  Both [size^3]. */
+int of_mc_count(const float* sdf, int32_t size, float level, int32_t* vert_count, int32_t* tri_count, void* stream);
+/* pass 2, after exclusive scans (of_exclusive_scan_i32) of both counts: verts [V, 3] fp32 and faces [F, 3] int32 of
+ * the grid, with V = vert_scan[size^3] and F = tri_scan[size^3]. */
+int of_mc_emit(const float* sdf, int32_t size, float level, const int32_t* vert_scan, const int32_t* tri_scan,
+               float* verts, int32_t* faces, void* stream);
+/* packed meshes: shape b has vertices verts[vert_offsets[b] .. vert_offsets[b+1]) and faces
+ * faces[face_offsets[b] .. face_offsets[b+1]) with shape-local vertex ids; offsets are int64 [batch + 1] on the device.
+ * bbox [batch, 6] = (min xyz, max xyz) of each shape's vertices (+inf / -inf for an empty shape). */
+int of_mesh_bbox(const float* verts, const int64_t* vert_offsets, int32_t batch, float* bbox, void* stream);
+/* trimesh sample_surface: per shape `count` points [batch, count, 3] fp32 and face_index [batch, count] int32.  The face
+ * is searchsorted(side='left') of u * total area in the fp64 inclusive prefix sum of the face areas (written to
+ * area_scan [face_offsets[batch]]), u in (0, 1], so zero-area faces are never chosen; the point is
+ * v0 + r1 (v1 - v0) + r2 (v2 - v0), with r1, r2 replaced by |r1 - 1|, |r2 - 1| when r1 + r2 > 1.  u (53 bits), r1
+ * and r2 (24 bits) come from Philox4x32-10 keyed by seed, counter (shape, sample): results depend on nothing else.  A
+ * shape without faces gets NaN points and face_index -1. */
+int of_surface_sample(const float* verts, const int64_t* vert_offsets, const int32_t* faces, const int64_t* face_offsets,
+                      int32_t batch, int32_t count, uint64_t seed, double* area_scan, float* points,
+                      int32_t* face_index, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -101,10 +101,15 @@ _PROTOS = {
     'of_chamfer_pairwise': (C.c_int, [_vp, _i32, _i32, _vp, _i32, _i32, _vp, _vp]),
     'of_match_cost': (C.c_int, [_vp, _vp, _i32, _i32, _vp, _vp, _vp]),
     'of_emd_cd_pairwise': (C.c_int, [_vp, _i32, _vp, _i32, _i32, _vp, _vp, _vp]),
+    'of_mc_count': (C.c_int, [_vp, _i32, _f32, _vp, _vp, _vp]),
+    'of_mc_emit': (C.c_int, [_vp, _i32, _f32, _vp, _vp, _vp, _vp, _vp]),
+    'of_mesh_bbox': (C.c_int, [_vp, _vp, _i32, _vp, _vp]),
+    'of_surface_sample': (C.c_int, [_vp, _vp, _vp, _vp, _i32, _i32, C.c_uint64, _vp, _vp, _vp, _vp]),
 }
 
 EMD_MAX_POINTS = 4096              # OF_EMD_MAX_POINTS
 CD_PAIRWISE_MAX_POINTS = 49152     # OF_CD_PAIRWISE_MAX_POINTS
+MC_MAX_SIZE = 512                  # OF_MC_MAX_SIZE
 
 EXPORTED_SYMBOLS = tuple(_PROTOS)
 

@@ -12,7 +12,8 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, 'csrc')
 LIBDIR = os.path.join(HERE, 'lib')
 LIB = os.path.join(LIBDIR, 'liboctfusion_b200.so')
-SOURCES = ['runtime.cu', 'gemm_simt.cu', 'gemm_tc.cu', 'norm.cu', 'attention.cu', 'misc.cu', 'graph.cu', 'mpu.cu', 'metrics.cu']
+SOURCES = ['runtime.cu', 'gemm_simt.cu', 'gemm_tc.cu', 'norm.cu', 'attention.cu', 'misc.cu', 'graph.cu', 'mpu.cu', 'metrics.cu',
+           'mesh.cu']
 NVCC_FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-O3', '-lineinfo', '-std=c++17',
               '-Xcompiler', '-fPIC', '--expt-relaxed-constexpr', '--extended-lambda']
 
@@ -34,7 +35,7 @@ def needs_build() -> bool:
     if not os.path.exists(LIB):
         return True
     t = os.path.getmtime(LIB)
-    deps = [os.path.join(CSRC, s) for s in SOURCES] + [os.path.join(CSRC, 'common.cuh'),
+    deps = [os.path.join(CSRC, s) for s in SOURCES + ['common.cuh', 'mc_table.inc']] + [
             os.path.join(HERE, '..', 'include', 'octfusion_b200.h'), os.path.abspath(__file__)]
     return any(os.path.getmtime(d) > t for d in deps)
 
