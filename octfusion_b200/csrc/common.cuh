@@ -43,12 +43,16 @@ template <> struct Elem<__nv_bfloat16> {
 };
 
 __device__ __forceinline__ float silu_f(float v) { return v / (1.0f + __expf(-v)); }
-// one MUFU op instead of two: x*sigmoid(x) = 0.5x(1 + tanh(x/2)); tanh.approx is good to ~2^-11, i.e. below
-// the bf16 rounding of the stored result (used for bf16 outputs only)
+// x * sigmoid(x) = x * rcp(1 + 2^(-x log2 e)) with two MUFU ops (used for bf16 outputs only).  Relative error below
+// 2^-16 for |x| < 128 (the rounding of -x log2 e dominates), far below the bf16 rounding of the stored result.  For
+// x < -87.3 the flushed reciprocal gives -0 where |silu(x)| < |x| 2^-126.  (0.5x(1 + tanh.approx(x/2)) is not
+// accurate enough: for x < 0, 1 + tanh is a difference near zero and tanh's 2^-11 error grows into a 1 % error at
+// x = -9 and a zero result below x ~ -17.)
 __device__ __forceinline__ float silu_fast(float v) {
-  float t;
-  asm("tanh.approx.f32 %0, %1;" : "=f"(t) : "f"(0.5f * v));
-  return 0.5f * v * (1.0f + t);
+  float e, r;
+  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e) : "f"(-1.4426950408889634f * v));
+  asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(1.0f + e));
+  return v * r;
 }
 
 // 8 bf16 <-> 8 floats through one 16-byte register quad

@@ -253,9 +253,9 @@ __global__ void __launch_bounds__(256, 5) gn_apply_kernel(GnSrc s, const float* 
       for (int i = 0; i < V; ++i) f[i] = FastAct<T>::silu(fmaf(f[i], sc[i], sh[i]));
     } else if (act == 2) {                                 // exact (erf) GELU = torch.nn.GELU() of the VAE heads
 #pragma unroll
-      for (int i = 0; i < V; ++i) {
-        const float v = fmaf(f[i], sc[i], sh[i]);
-        f[i] = 0.5f * v * (1.0f + erff(v * 0.70710678118654752f));
+      for (int i = 0; i < V; ++i) {                        // 1 + erf(x) = erfc(-x): erfc keeps the relative accuracy
+        const float v = fmaf(f[i], sc[i], sh[i]);          // of the negative tail, where 1 + erff(x) cancels (x < -2)
+        f[i] = 0.5f * v * erfcf(v * -0.70710678118654752f);
       }
     } else {
 #pragma unroll
