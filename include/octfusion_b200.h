@@ -75,7 +75,6 @@ typedef struct of_gemm_args {
   const int32_t* in_rows;                        /* identity mode only, may be NULL           */
   int32_t taps;
   const uint8_t* node_type; int32_t ntype;       /* ntype = 0: no one-hot columns             */
-  int32_t a_silu;                                /* fp32 path only: apply SiLU to A on load   */
   /* B: fp32 path  -> canonical fp32 [K, N] row-major, K = taps*(c0+c1+ntype), k = tap*(c0+c1+ntype)+c
    *    (exactly GraphConv.weights; other layouts go through of_repack_weight once)
    *    tensor-core path -> bf16 tile image produced by of_pack_weight_tc                         */
@@ -90,13 +89,8 @@ typedef struct of_gemm_args {
   int32_t dtype;                                 /* activation dtype of a0/a1/resid/out       */
   /* tensor-core path only: slots with several neighbours read their pre-averaged row.  There tap_tab uses
    * the ORDINAL encoding of of_graph_multi_index: v <= -2 -> row -(v+2) of a_multi (built per input tensor
-   * by of_gather_mean_rows); multi_types[ord] = per-type neighbour counts, 8 bits per type -- only read when
-   * nt_block is NULL, and only exact while a slot has < 256 neighbours of one type (two adaptive levels: <= 16;
-   * deeper octrees such as the VAE's depth 8 must pass nt_block).                                       */
+   * by of_gather_mean_rows).                                                                                 */
   const void* a_multi; int64_t ld_multi;
-  const uint64_t* multi_types;
-  /* row counts of a0 / a1 (informational; may be 0)                                                          */
-  int32_t rows_a0, rows_a1;
   /* tensor-core path with ntype > 0 (required there): the node-type K block as a precomputed bf16 [M, 64] tensor
    * (of_graph_type_block, record-encoded table)                                                              */
   const void* nt_block;
@@ -126,14 +120,6 @@ int of_gather_gemm_simt(const of_gemm_args* args, void* stream);
 /* Tensor-core path (wgmma, bf16 operands, fp32 accumulate). Requires dtype = OF_BF16,
  * (c0 % 64 == 0), (c1 % 64 == 0), N % 16 == 0 and w packed by of_pack_weight_tc. */
 int of_gather_gemm_tc(const of_gemm_args* args, void* stream);
-/* Split-K variant for launches whose row tiles cannot fill the GPU (the dense 4^3 / 8^3 levels: M = 2048 at B = 32, with
- * K up to 13824): of_tc_splitk_plan returns the number S of K ranges this library would use for `args` (1 = do not
- * split).  With S > 1 the caller provides a workspace of S * M * N floats and calls of_gather_gemm_tc_splitk: pass 1
- * runs the same tensor-core kernel over (output tile, K range) pairs writing fp32 partial sums, pass 2 adds the ranges in
- * order (bit-reproducible) with bias / row_add / resid, stores `out` and computes the stat_out statistics.  Same
- * arguments and results as of_gather_gemm_tc up to fp32 summation order. */
-int of_tc_splitk_plan(const of_gemm_args* args);
-int of_gather_gemm_tc_splitk(const of_gemm_args* args, int32_t splits, float* workspace, void* stream);
 /* size in bytes of the packed image for K_feat = taps*(c0+c1) feature rows + ntype one-hot rows */
 int64_t of_pack_weight_tc_bytes(int32_t taps, int32_t c, int32_t ntype, int32_t N);
 /* w_canonical: fp32 [taps*(c+ntype), N]; out: packed bf16 image */
@@ -268,13 +254,11 @@ int of_graph_fill(const of_octree_levels* oct, int32_t D, const int32_t* need_of
 /* Multi-neighbour slots (coarse leaf next to a subdivided cell: 4..16 finer neighbours, averaged by
  * scatter_mean, utils/scatter.py:42-66; up to 4^k for k adaptive levels).  of_graph_multi_flags marks them (flags[i] = tap_tab[i] <= -2);
  * after an exclusive scan of the flags, of_graph_multi_index writes the ordinal-encoded table used by the
- * tensor-core path (v <= -2 -> -(ordinal+2)), multi_off[ord] = offset of the slot's record in tap_extra, and
- * multi_types[ord] = packed per-type neighbour counts (8 bits per node type).
+ * tensor-core path (v <= -2 -> -(ordinal+2)) and multi_off[ord] = offset of the slot's record in tap_extra.
  * of_gather_mean_rows: out[ord, :] = mean over the slot's neighbours of (a0|a1)[row, :]  (per input tensor). */
 int of_graph_multi_flags(const int32_t* tap_tab, int64_t slots, int32_t* flags, void* stream);
-int of_graph_multi_index(const int32_t* tap_tab, const int32_t* tap_extra, const uint8_t* node_type,
-                         int64_t slots, const int32_t* flag_scan, int32_t* tap_tab_ord, int32_t* multi_off,
-                         uint64_t* multi_types, void* stream);
+int of_graph_multi_index(const int32_t* tap_tab, const int32_t* tap_extra, int64_t slots, const int32_t* flag_scan,
+                         int32_t* tap_tab_ord, int32_t* multi_off, void* stream);
 /* Node-type K block of the tensor-core GEMM, a per-graph constant: out [rows, 64] bf16, column tap*ntype + type =
  * (#neighbours of that type in slot (row, tap)) / (#neighbours) = the scatter_mean of the one-hot columns that
  * GraphConv.forward appends to the features (models/networks/modules.py:199-202, 208-210); zero elsewhere.

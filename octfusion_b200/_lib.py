@@ -24,7 +24,6 @@ class GemmArgs(C.Structure):
         ('in_rows', _vp),
         ('taps', _i32),
         ('node_type', _vp), ('ntype', _i32),
-        ('a_silu', _i32),
         ('w', _vp),
         ('bias', _vp),
         ('row_add', _vp), ('ld_row_add', _i64), ('row_add_idx', _vp),
@@ -35,8 +34,6 @@ class GemmArgs(C.Structure):
         ('M', _i32), ('N', _i32),
         ('dtype', _i32),
         ('a_multi', _vp), ('ld_multi', _i64),
-        ('multi_types', _vp),
-        ('rows_a0', _i32), ('rows_a1', _i32),
         ('nt_block', _vp),
         ('reverse', _i32),
         ('stat_out', _vp), ('stat_chunk_seg', _vp), ('stat_seg_slot', _vp), ('stat_sample', _vp),
@@ -62,8 +59,6 @@ _PROTOS = {
     'of_abi_sizeof_octree_levels': (C.c_int, []),
     'of_gather_gemm_simt': (C.c_int, [C.POINTER(GemmArgs), _vp]),
     'of_gather_gemm_tc': (C.c_int, [C.POINTER(GemmArgs), _vp]),
-    'of_tc_splitk_plan': (C.c_int, [C.POINTER(GemmArgs)]),
-    'of_gather_gemm_tc_splitk': (C.c_int, [C.POINTER(GemmArgs), _i32, _vp, _vp]),
     'of_pack_weight_tc_bytes': (_i64, [_i32, _i32, _i32, _i32]),
     'of_pack_weight_tc': (C.c_int, [_vp, _i32, _i32, _i32, _i32, _vp, _vp]),
     'of_repack_weight': (C.c_int, [_vp, _i64, _i64, _i64, _i32, _i32, _i32, _vp, _vp]),
@@ -88,7 +83,7 @@ _PROTOS = {
     'of_graph_fill': (C.c_int, [C.POINTER(OctreeLevels), _i32, _vp, _vp, _vp, _vp, _vp, _vp]),
     'of_histogram_i32': (C.c_int, [_vp, _i64, _i32, _vp, _vp]),
     'of_graph_multi_flags': (C.c_int, [_vp, _i64, _vp, _vp]),
-    'of_graph_multi_index': (C.c_int, [_vp, _vp, _vp, _i64, _vp, _vp, _vp, _vp, _vp]),
+    'of_graph_multi_index': (C.c_int, [_vp, _vp, _i64, _vp, _vp, _vp, _vp]),
     'of_graph_type_block': (C.c_int, [_vp, _vp, _vp, _i64, _i32, _i32, _vp, _vp]),
     'of_gather_mean_rows': (C.c_int, [_vp, _i64, _i32, _vp, _i64, _i32, _vp, _vp, _i32, _i32, _vp, _i64, _vp]),
     'of_graph_edge_count': (C.c_int, [_vp, _vp, _i64, _vp, _vp]),
@@ -118,7 +113,7 @@ class LibraryMissing(ImportError):
     pass
 
 
-ABI_VERSION = 5          # of_version() of the header this binding mirrors
+ABI_VERSION = 6          # of_version() of the header this binding mirrors
 
 
 def _load():

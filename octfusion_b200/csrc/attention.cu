@@ -9,7 +9,6 @@
 // qkv is channels-last [B*T, 3C] with the reference's legacy head-major split: head h owns
 // columns [h*3ch, (h+1)*3ch) = q | k | v (modules.py:531,540-541).
 #include "common.cuh"
-#include <stdlib.h>
 
 namespace of {
 
@@ -308,20 +307,16 @@ extern "C" int of_attention(const void* qkv, int64_t ld_qkv, void* out, int64_t 
   OF_REQUIRE(dtype == OF_F32 || dtype == OF_BF16, "of_attention: bad dtype");
   OF_REQUIRE(ch % 4 == 0, "of_attention: ch must be a multiple of 4");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  {
-    static int force_simt = -1;                            // OCTFUSION_ATT_SIMT=1: CUDA-core kernel for every shape
-    if (force_simt < 0) { const char* e = getenv("OCTFUSION_ATT_SIMT"); force_simt = e ? atoi(e) : 0; }
-    // tensor-core path: bf16, 16-byte aligned rows
-    if (dtype == OF_BF16 && !force_simt && (ch == 16 || ch == 32 || ch == 64 || ch == 128) && ld_qkv % 8 == 0 && ld_out % 2 == 0 &&
-        reinterpret_cast<uintptr_t>(qkv) % 16 == 0 && reinterpret_cast<uintptr_t>(out) % 4 == 0) {
-      int rc = ch == 16 ? launch_attention_tc<16>(qkv, ld_qkv, out, ld_out, batch, tokens, heads, st)
-             : ch == 32 ? launch_attention_tc<32>(qkv, ld_qkv, out, ld_out, batch, tokens, heads, st)
-             : ch == 64 ? launch_attention_tc<64>(qkv, ld_qkv, out, ld_out, batch, tokens, heads, st)
-                        : launch_attention_tc<128>(qkv, ld_qkv, out, ld_out, batch, tokens, heads, st);
-      if (rc == OF_OK) {
-        OF_LAUNCH_CHECK("of_attention(tc)");
-        return OF_OK;
-      }
+  // tensor-core path: bf16, 16-byte aligned rows
+  if (dtype == OF_BF16 && (ch == 16 || ch == 32 || ch == 64 || ch == 128) && ld_qkv % 8 == 0 && ld_out % 2 == 0 &&
+      reinterpret_cast<uintptr_t>(qkv) % 16 == 0 && reinterpret_cast<uintptr_t>(out) % 4 == 0) {
+    int rc = ch == 16 ? launch_attention_tc<16>(qkv, ld_qkv, out, ld_out, batch, tokens, heads, st)
+           : ch == 32 ? launch_attention_tc<32>(qkv, ld_qkv, out, ld_out, batch, tokens, heads, st)
+           : ch == 64 ? launch_attention_tc<64>(qkv, ld_qkv, out, ld_out, batch, tokens, heads, st)
+                      : launch_attention_tc<128>(qkv, ld_qkv, out, ld_out, batch, tokens, heads, st);
+    if (rc == OF_OK) {
+      OF_LAUNCH_CHECK("of_attention(tc)");
+      return OF_OK;
     }
   }
   const size_t smem = ((size_t)2 * tokens * (ch + 4) + (size_t)ATT_WARPS * tokens * ATT_QB + (size_t)ATT_WARPS * ATT_QB * ch) * 4;

@@ -16,15 +16,9 @@ namespace of {
 
 template <typename T>
 __device__ __forceinline__ float load_feat(const of_gemm_args& p, int src, int c) {
-  float v;
-  if (c < p.c0) {
-    v = Elem<T>::ld(reinterpret_cast<const T*>(p.a0) + (int64_t)src * p.lda0 + c);
-  } else if (c < p.c0 + p.c1) {
-    v = Elem<T>::ld(reinterpret_cast<const T*>(p.a1) + (int64_t)src * p.lda1 + (c - p.c0));
-  } else {
-    return p.node_type[src] == (uint8_t)(c - p.c0 - p.c1) ? 1.0f : 0.0f;
-  }
-  return p.a_silu ? silu_f(v) : v;
+  if (c < p.c0) return Elem<T>::ld(reinterpret_cast<const T*>(p.a0) + (int64_t)src * p.lda0 + c);
+  if (c < p.c0 + p.c1) return Elem<T>::ld(reinterpret_cast<const T*>(p.a1) + (int64_t)src * p.lda1 + (c - p.c0));
+  return p.node_type[src] == (uint8_t)(c - p.c0 - p.c1) ? 1.0f : 0.0f;
 }
 
 template <typename T>

@@ -10,7 +10,7 @@
 // directly in shared memory, in the 128-byte-swizzled K-major layout wgmma reads.
 //
 // One persistent CTA per SM, launched as clusters of two for BN >= 128 (TcCfg::CLUSTER): the CTAs of a pair compute two
-// adjacent 128-row tiles of the same columns and K range, so they need the same weight tiles, and each fetches half of
+// adjacent 128-row tiles of the same columns, so they need the same weight tiles, and each fetches half of
 // every weight tile for both.
 // 384 threads = three warpgroups:
 //   warpgroup 0    producers: each warp fills every PW-th stage of the shared-memory ring (PW = 4, or the ring depth
@@ -33,7 +33,6 @@
 // from a per-graph precomputed tensor (of_graph_type_block); slots with several finer neighbours read a
 // pre-averaged row (of_gather_mean_rows); the weights are re-laid once by of_pack_weight_tc.
 #include "common.cuh"
-#include <stdlib.h>
 #include <string.h>
 #include <type_traits>
 
@@ -258,14 +257,13 @@ struct TcCfg {
   static_assert(B_BYTES % 32 == 0, "each CTA of a pair copies one 16-byte-aligned half of the weight tile");
 };
 
+// (Field order matters to ptxas: with npad ahead of the tile counts, <256> spills 20 B more in the epilogue.)
 struct TcParams {
   of_gemm_args g;
-  int num_kb;        // K blocks per (virtual) tile = all K blocks / ksplit
-  int ksplit;        // split-K: every output tile is computed as ksplit virtual tiles over consecutive K ranges, each
-                     // writing fp32 partial sums to its own [M, N] slab of the workspace (of_gather_gemm_tc_splitk)
+  int num_kb;        // K blocks per tile
   int cblocks;       // (c0+c1)/64
-  int npad;          // N rounded up to 16 (rows per K block in the packed weight image)
   int m_tiles, n_tiles;
+  int npad;          // N rounded up to 16 (rows per K block in the packed weight image)
 };
 
 // Sum of a[0..NV-1] (NV = 16 or 32) over the 32 lanes of the warp by recursive halving: NV = 16: 8+4+2+1+1 = 16 shuffles,
@@ -306,15 +304,13 @@ __global__ void __launch_bounds__(TC_THREADS, 1) gather_gemm_tc_kernel(const __g
   const int warp = t >> 5, lane = t & 31;
   const of_gemm_args& g = p.g;
   const int taps = g.taps;
-  const int ksplit = p.ksplit;
-  // CTA pairs (Cfg::CLUSTER = 2): a work unit is (two adjacent 128-row M tiles, N tile, K range); CTA `rank` of the
-  // cluster takes M tile 2 * pair + rank, both walk the same units and K blocks, and each copies one half of the shared
-  // weight tile into both.  With single CTAs a unit is one M tile.  Virtual unit v: output unit v / ksplit, K range
-  // v % ksplit.
+  // CTA pairs (Cfg::CLUSTER = 2): a work unit is (two adjacent 128-row M tiles, N tile); CTA `rank` of the cluster takes
+  // M tile 2 * pair + rank, both walk the same units and K blocks, and each copies one half of the shared weight tile
+  // into both.  With single CTAs a unit is one M tile.
   constexpr int CL = Cfg::CLUSTER;
   const int rank = CL == 2 ? (int)cluster_ctarank() : 0;
   const int cid = (int)cluster_id_x(), nclusters = (int)cluster_count_x();
-  const int total_units = (p.m_tiles + CL - 1) / CL * p.n_tiles * ksplit;
+  const int total_units = (p.m_tiles + CL - 1) / CL * p.n_tiles;
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < Cfg::STAGES; ++s) {
@@ -338,14 +334,13 @@ __global__ void __launch_bounds__(TC_THREADS, 1) gather_gemm_tc_kernel(const __g
       const int my_units = (total_units - cid + nclusters - 1) / nclusters;
       const int total_stages = my_units * p.num_kb;
       struct Pos { int m0, n0, kabs; };
-      // stage s of this CTA -> rows, columns and ABSOLUTE K block (split-K: the K range's offset included); the rows
-      // of the second CTA of the last pair lie beyond M when the number of M tiles is odd
+      // stage s of this CTA -> rows, columns and K block; the rows of the second CTA of the last pair lie beyond M when
+      // the number of M tiles is odd
       auto pos_of = [&](int s) {
         const int ui = s / p.num_kb, kb = s - ui * p.num_kb;
         const int unit = cid + ui * nclusters;
         const int vunit = g.reverse ? total_units - 1 - unit : unit;
-        const int ptile = vunit / ksplit;
-        return Pos{((ptile / p.n_tiles) * CL + rank) * TC_BM, (ptile % p.n_tiles) * BN, (vunit - ptile * ksplit) * p.num_kb + kb};
+        return Pos{((vunit / p.n_tiles) * CL + rank) * TC_BM, (vunit % p.n_tiles) * BN, kb};
       };
       auto fetch_taps = [&](const Pos& c, int32_t (&tv)[32]) {
         const int cb = c.kabs / taps;
@@ -447,9 +442,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) gather_gemm_tc_kernel(const __g
     };
     for (int unit = cid; unit < total_units; unit += nclusters) {
       const int vunit = g.reverse ? total_units - 1 - unit : unit;
-      const int ptile = vunit / ksplit;
-      const int64_t split_row0 = (int64_t)(vunit - ptile * ksplit) * g.M;        // this K range's slab of the workspace
-      const int m0 = ((ptile / p.n_tiles) * CL + rank) * TC_BM, n0 = (ptile % p.n_tiles) * BN;
+      const int m0 = ((vunit / p.n_tiles) * CL + rank) * TC_BM, n0 = (vunit % p.n_tiles) * BN;
 #pragma unroll
       for (int i = 0; i < BN / 2; ++i) fence_operand(acc[i]);
       int prev = 0;
@@ -489,7 +482,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) gather_gemm_tc_kernel(const __g
       const uint32_t stg = stg_base + (uint32_t)cw * 64 * Cfg::EPI_LD * 4;
       const int m = m0 + cw * 64 + rl;
       const bool row_ok = m < g.M;
-      const int64_t orow = row_ok ? (g.out_rows ? (int64_t)g.out_rows[m] : (int64_t)m + split_row0) : 0;
+      const int64_t orow = row_ok ? (g.out_rows ? (int64_t)g.out_rows[m] : (int64_t)m) : 0;
       const float* radd = (row_ok && g.row_add) ? g.row_add + (int64_t)g.row_add_idx[m] * g.ld_row_add : nullptr;
       const __nv_bfloat16* res =
           (row_ok && g.resid) ? reinterpret_cast<const __nv_bfloat16*>(g.resid) + (int64_t)m * g.ld_resid : nullptr;
@@ -747,7 +740,7 @@ static int launch_tc(TcParams& p, cudaStream_t st) {
   }
   p.m_tiles = (p.g.M + TC_BM - 1) / TC_BM;
   p.n_tiles = p.npad / BN;
-  const int units = (p.m_tiles + Cfg::CLUSTER - 1) / Cfg::CLUSTER * p.n_tiles * p.ksplit;
+  const int units = (p.m_tiles + Cfg::CLUSTER - 1) / Cfg::CLUSTER * p.n_tiles;
   cfg.gridDim = dim3(Cfg::CLUSTER * (units < clusters ? units : clusters));
   const cudaError_t e = cudaLaunchKernelEx(&cfg, gather_gemm_tc_kernel<BN>, p);
   if (e != cudaSuccess) {
@@ -798,16 +791,14 @@ extern "C" int of_pack_weight_tc(const float* w_canonical, int32_t taps, int32_t
   return OF_OK;
 }
 
-// ksplit > 1 (of_gather_gemm_tc_splitk): K is cut into ksplit equal ranges of whole K blocks, the virtual tile (output
-// tile, range) writes its fp32 partial sums into slab `range` of args->out ([ksplit][M][N] fp32, no epilogue extras)
-static int run_tc(const of_gemm_args* args, int ksplit, void* stream) {
+extern "C" int of_gather_gemm_tc(const of_gemm_args* args, void* stream) {
   int rc = check_gemm_args(args, "of_gather_gemm_tc");
   if (rc) return rc;
   const of_gemm_args& a = *args;
   if (a.dtype != OF_BF16 || a.c0 % 64 != 0 || a.c1 % 64 != 0 || a.taps > TC_MAX_TAPS || a.taps * a.ntype > 64 ||
-      a.ntype > 8 || a.a_silu) {
-    set_error("of_gather_gemm_tc: unsupported (dtype=%d c0=%d c1=%d taps=%d ntype=%d a_silu=%d)", a.dtype, a.c0, a.c1,
-              a.taps, a.ntype, a.a_silu);
+      a.ntype > 8) {
+    set_error("of_gather_gemm_tc: unsupported (dtype=%d c0=%d c1=%d taps=%d ntype=%d)", a.dtype, a.c0, a.c1, a.taps,
+              a.ntype);
     return OF_E_UNSUPPORTED;
   }
   if (a.ntype > 0 && a.nt_block == nullptr) {
@@ -828,17 +819,8 @@ static int run_tc(const of_gemm_args* args, int ksplit, void* stream) {
   p.g = a;
   p.cblocks = (a.c0 + a.c1) / 64;
   p.num_kb = p.cblocks * a.taps + (a.ntype > 0 ? 1 : 0);
-  p.ksplit = 1;
   p.npad = (a.N + 15) / 16 * 16;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  if (ksplit > 1) {
-    OF_REQUIRE(p.num_kb % ksplit == 0 && p.npad % 32 == 0 && a.N == p.npad && a.out_rows == nullptr && a.out_f32 == 1 &&
-                   a.bias == nullptr && a.row_add == nullptr && a.resid == nullptr && a.stat_out == nullptr,
-               "of_gather_gemm_tc_splitk: internal argument error");
-    p.ksplit = ksplit;
-    p.num_kb /= ksplit;
-    return launch_tc_bn(p.npad % 256 == 0 ? 256 : p.npad % 128 == 0 ? 128 : p.npad % 64 == 0 ? 64 : 32, p, st);
-  }
   if (p.npad % 32 != 0) return launch_tc<16>(p, st);
   // Small M (the dense 4^3 / 8^3 levels: 2048 / 16384 rows): the widest tile would leave most SMs idle (16 row tiles of 128
   // rows for 132 SMs) with every CTA walking the whole K loop alone.  Take the widest tile shape whose tile count still
@@ -858,131 +840,4 @@ static int run_tc(const of_gemm_args* args, int ksplit, void* stream) {
     if (t >= enough) break;
   }
   return launch_tc_bn(bn, p, st);
-}
-
-extern "C" int of_gather_gemm_tc(const of_gemm_args* args, void* stream) { return run_tc(args, 1, stream); }
-
-namespace of {
-
-// Second pass of a split-K GEMM: out[m, :] = sum over the K ranges (in range order: bit-reproducible) of the fp32 partial
-// slabs + bias + emb[sample] + residual, stored in the activation dtype, and -- like the single-pass epilogue -- the
-// group-norm partial statistics of the fp32 values before rounding.  One CTA per (32-row chunk, 128 columns): warp w owns
-// row w of the chunk, lane l its columns 4l..4l+3 (coalesced 16-byte loads of every slab); the per-row (sum, sum of
-// squares) of each granule go through shared memory and warp 0 adds the chunk's rows in row order, starting a new
-// statistics segment at every change of sample id (the scheme of gn_stats_kernel, csrc/norm.cu).
-template <int GRAN>
-__global__ void __launch_bounds__(1024) splitk_reduce_kernel(of_gemm_args g, const float* __restrict__ ws, int splits) {
-  constexpr int G = 4 / GRAN;                               // granules per thread
-  __shared__ float part[32][32][G][2];
-  const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int64_t chunk = blockIdx.x;
-  const int64_t r = chunk * 32 + w;
-  const int cv = blockIdx.y * 128 + lane * 4;
-  const bool col_ok = cv < g.N;
-  const bool st = g.stat_out != nullptr;
-  float sum[G], sq[G];
-#pragma unroll
-  for (int i = 0; i < G; ++i) { sum[i] = 0.0f; sq[i] = 0.0f; }
-  if (r < g.M && col_ok) {
-    const int64_t slab = (int64_t)g.M * g.N;
-    const float* src = ws + r * g.N + cv;
-    float4 v = *reinterpret_cast<const float4*>(src);
-    for (int sidx = 1; sidx < splits; ++sidx) {
-      const float4 t = *reinterpret_cast<const float4*>(src + sidx * slab);
-      v.x += t.x; v.y += t.y; v.z += t.z; v.w += t.w;
-    }
-    if (g.bias != nullptr) { v.x += g.bias[cv]; v.y += g.bias[cv + 1]; v.z += g.bias[cv + 2]; v.w += g.bias[cv + 3]; }
-    if (g.row_add != nullptr) {
-      const float* e = g.row_add + (int64_t)g.row_add_idx[r] * g.ld_row_add + cv;
-      v.x += e[0]; v.y += e[1]; v.z += e[2]; v.w += e[3];
-    }
-    if (g.resid != nullptr) {
-      const __nv_bfloat16* q = reinterpret_cast<const __nv_bfloat16*>(g.resid) + r * g.ld_resid + cv;
-      v.x += __bfloat162float(q[0]); v.y += __bfloat162float(q[1]); v.z += __bfloat162float(q[2]); v.w += __bfloat162float(q[3]);
-    }
-    if (g.out_f32) {
-      float* o = reinterpret_cast<float*>(g.out) + r * g.ldo + cv;
-      o[0] = v.x; o[1] = v.y; o[2] = v.z; o[3] = v.w;
-    } else {
-      __nv_bfloat16* o = reinterpret_cast<__nv_bfloat16*>(g.out) + r * g.ldo + cv;
-      o[0] = __float2bfloat16_rn(v.x); o[1] = __float2bfloat16_rn(v.y); o[2] = __float2bfloat16_rn(v.z); o[3] = __float2bfloat16_rn(v.w);
-    }
-    const float f[4] = {v.x, v.y, v.z, v.w};
-#pragma unroll
-    for (int i = 0; i < 4; ++i) { sum[i / GRAN] += f[i]; sq[i / GRAN] = fmaf(f[i], f[i], sq[i / GRAN]); }
-  }
-  if (!st) return;
-#pragma unroll
-  for (int i = 0; i < G; ++i) { part[w][lane][i][0] = sum[i]; part[w][lane][i][1] = sq[i]; }
-  __syncthreads();
-  if (w != 0 || !col_ok) return;
-  const int64_t r0 = chunk * 32;
-  const int64_t r1 = r0 + 32 < g.M ? r0 + 32 : (int64_t)g.M;
-  const int half = g.N / GRAN * 2;
-  auto sample_of = [&](int64_t row) { return g.stat_sample ? g.stat_sample[row] : (int)(row / g.stat_rows_per_sample); };
-  int seg = g.stat_chunk_seg[chunk];
-  int cur = sample_of(r0);
-  float ts[G], tq[G];
-#pragma unroll
-  for (int i = 0; i < G; ++i) { ts[i] = 0.0f; tq[i] = 0.0f; }
-  auto flush = [&]() {
-#pragma unroll
-    for (int i = 0; i < G; ++i) {
-      *reinterpret_cast<float2*>(g.stat_out + (int64_t)g.stat_seg_slot[seg] * half + (cv / GRAN + i) * 2) = make_float2(ts[i], tq[i]);
-      ts[i] = 0.0f; tq[i] = 0.0f;
-    }
-  };
-  for (int64_t row = r0; row < r1; ++row) {
-    const int b = sample_of(row);
-    if (b != cur) { flush(); ++seg; cur = b; }
-#pragma unroll
-    for (int i = 0; i < G; ++i) { ts[i] += part[row - r0][lane][i][0]; tq[i] += part[row - r0][lane][i][1]; }
-  }
-  flush();
-}
-
-// How many K ranges of_gather_gemm_tc_splitk should use for this launch (1 = do not split): only for launches whose
-// 128-row tiles cannot fill half of the SMs, whole K blocks per range, at least 4 per range, at most one wave of CTAs.
-static int splitk_plan(const of_gemm_args& a) {
-  if (a.dtype != OF_BF16 || a.c0 % 64 != 0 || a.c1 % 64 != 0 || a.N % 32 != 0 || a.out_rows != nullptr || a.M <= 0 ||
-      a.a_silu || (a.ntype > 0 && a.nt_block == nullptr))
-    return 1;
-  const int num_kb = (a.c0 + a.c1) / 64 * a.taps + (a.ntype > 0 ? 1 : 0);
-  const int bn = a.N % 256 == 0 ? 256 : a.N % 128 == 0 ? 128 : a.N % 64 == 0 ? 64 : 32;
-  const int64_t tiles = (int64_t)((a.M + 127) / 128) * (a.N / bn);
-  const int sms = num_sms();
-  if (tiles * 2 > sms) return 1;
-  int best = 1;
-  for (int d = 2; d <= num_kb / 4 && tiles * d <= sms; ++d)
-    if (num_kb % d == 0) best = d;
-  return best;
-}
-
-}  // namespace of
-
-extern "C" int of_tc_splitk_plan(const of_gemm_args* args) {
-  if (args == nullptr) return 1;
-  return of::splitk_plan(*args);
-}
-
-extern "C" int of_gather_gemm_tc_splitk(const of_gemm_args* args, int32_t splits, float* workspace, void* stream) {
-  OF_REQUIRE(args != nullptr && workspace != nullptr && splits >= 2, "of_gather_gemm_tc_splitk: bad arguments");
-  OF_REQUIRE(splits == of::splitk_plan(*args), "of_gather_gemm_tc_splitk: splits=%d is not the plan for this launch", splits);
-  const of_gemm_args& a = *args;
-  if (a.stat_out != nullptr) {
-    OF_REQUIRE(a.stat_chunk_seg != nullptr && a.stat_seg_slot != nullptr && (a.stat_sample != nullptr || a.stat_rows_per_sample > 0),
-               "of_gather_gemm_tc_splitk: stat_out needs stat_chunk_seg, stat_seg_slot and a sample map");
-  }
-  OF_REQUIRE((a.row_add == nullptr) == (a.row_add_idx == nullptr), "of_gather_gemm_tc_splitk: row_add and row_add_idx go together");
-  of_gemm_args part = a;                                   // pass 1: plain fp32 partial sums into the workspace slabs
-  part.out = workspace; part.ldo = a.N; part.out_f32 = 1;
-  part.bias = nullptr; part.row_add = nullptr; part.row_add_idx = nullptr; part.resid = nullptr; part.stat_out = nullptr;
-  int rc = run_tc(&part, splits, stream);
-  if (rc) return rc;
-  const dim3 grid((unsigned)((a.M + 31) / 32), (unsigned)((a.N + 127) / 128));
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  if (a.N % 128 == 0) of::splitk_reduce_kernel<4><<<grid, 1024, 0, st>>>(a, workspace, splits);
-  else of::splitk_reduce_kernel<2><<<grid, 1024, 0, st>>>(a, workspace, splits);
-  OF_LAUNCH_CHECK("of_gather_gemm_tc_splitk (reduce)");
-  return OF_OK;
 }

@@ -326,22 +326,15 @@ __global__ void multi_flags_kernel(const int32_t* __restrict__ tab, int64_t slot
   if (i < slots) flags[i] = tab[i] <= -2 ? 1 : 0;
 }
 
-__global__ void multi_index_kernel(const int32_t* __restrict__ tab, const int32_t* __restrict__ extra,
-                                   const uint8_t* __restrict__ node_type, int64_t slots,
-                                   const int32_t* __restrict__ scan, int32_t* __restrict__ tab_ord,
-                                   int32_t* __restrict__ multi_off, unsigned long long* __restrict__ multi_types) {
+__global__ void multi_index_kernel(const int32_t* __restrict__ tab, int64_t slots, const int32_t* __restrict__ scan,
+                                   int32_t* __restrict__ tab_ord, int32_t* __restrict__ multi_off) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= slots) return;
   const int32_t v = tab[i];
   if (v > -2) { tab_ord[i] = v; return; }
   const int32_t ord = scan[i];
-  const int32_t o = -(v + 2);
   tab_ord[i] = -(ord + 2);
-  multi_off[ord] = o;
-  const int n = extra[o];
-  unsigned long long packed = 0ull;
-  for (int k = 1; k <= n; ++k) packed += 1ull << (8 * (node_type ? node_type[extra[o + k]] : 0));
-  multi_types[ord] = packed;
+  multi_off[ord] = -(v + 2);
 }
 
 // Node-type K block of the tensor-core GEMM, precomputed once per graph: row m, column tap*ntype + type holds
@@ -431,15 +424,13 @@ extern "C" int of_graph_multi_flags(const int32_t* tap_tab, int64_t slots, int32
   return OF_OK;
 }
 
-extern "C" int of_graph_multi_index(const int32_t* tap_tab, const int32_t* tap_extra, const uint8_t* node_type,
-                                    int64_t slots, const int32_t* flag_scan, int32_t* tap_tab_ord, int32_t* multi_off,
-                                    uint64_t* multi_types, void* stream) {
-  OF_REQUIRE(tap_tab && tap_extra && flag_scan && tap_tab_ord && multi_off && multi_types && slots >= 0,
+extern "C" int of_graph_multi_index(const int32_t* tap_tab, const int32_t* tap_extra, int64_t slots,
+                                    const int32_t* flag_scan, int32_t* tap_tab_ord, int32_t* multi_off, void* stream) {
+  OF_REQUIRE(tap_tab && tap_extra && flag_scan && tap_tab_ord && multi_off && slots >= 0,
              "of_graph_multi_index: bad arguments");
   if (slots == 0) return OF_OK;
   multi_index_kernel<<<(unsigned)((slots + 255) / 256), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
-      tap_tab, tap_extra, node_type, slots, flag_scan, tap_tab_ord, multi_off,
-      reinterpret_cast<unsigned long long*>(multi_types));
+      tap_tab, slots, flag_scan, tap_tab_ord, multi_off);
   OF_LAUNCH_CHECK("of_graph_multi_index");
   return OF_OK;
 }

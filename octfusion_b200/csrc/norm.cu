@@ -305,11 +305,10 @@ static bool vec_ok(const void* p, int64_t ld, int c, int v, int esz) {
 }
 
 // rows per CTA: a fixed number of BYTES per CTA (so that every thread streams enough rows to amortise the
-// prologue/epilogue latency chain), at least 256 rows.  OCTFUSION_GN_CHUNK_KB overrides (experiments).
+// prologue/epilogue latency chain), at least 256 rows.
 static int gn_chunk_rows(int C, int esz) {
-  static int kb = -1;
-  if (kb < 0) { const char* e = getenv("OCTFUSION_GN_CHUNK_KB"); kb = e ? atoi(e) : 64; }
-  int64_t rows = ((int64_t)kb * 1024) / ((int64_t)C * esz);
+  constexpr int64_t CHUNK_BYTES = 64 * 1024;
+  int64_t rows = CHUNK_BYTES / ((int64_t)C * esz);
   rows = (rows / 256) * 256;
   return (int)(rows < 256 ? 256 : rows);
 }

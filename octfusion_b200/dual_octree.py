@@ -135,7 +135,7 @@ class DualOctree:
         counts = torch.cat(pending).tolist()                                      # sync 2
         for i, D in enumerate(depths):
             p = self.plan[D]
-            p.tap.multi_finish(counts[2 * i], p.node_type)
+            p.tap.multi_finish(counts[2 * i])
             p.stat.finish(counts[2 * i + 1])
         # ---- row maps of GraphDownsample / GraphUpsample (reference modules.py:409-428, 458-472) ----
         ar = lambda n: torch.arange(n, dtype=torch.int32, device=dev)  # noqa: E731

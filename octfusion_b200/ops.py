@@ -5,13 +5,12 @@ torch is used for device memory (torch.empty / zeros), streams and nothing else.
 """
 from __future__ import annotations
 import ctypes as C
-import os
 import torch
 
 from . import _lib
 from ._lib import lib, ptr, stream, check, dt, GemmArgs
 
-_FORCE_SIMT = os.environ.get('OCTFUSION_B200_FORCE_SIMT', '0') == '1'
+_FORCE_SIMT = False
 _PROFILE = None        # when a list: (kind, meta, start_event, end_event) per GEMM launch (bench.py roofline leg)
 
 
@@ -45,15 +44,15 @@ def set_force_simt(flag: bool):
 
 class TapTable:
     """Neighbour table of the tap-gather GEMM (see include/octfusion_b200.h).
-    tab/extra: record encoding (CUDA-core path).  tab_ord/multi_off/multi_types: ordinal encoding of the
-    multi-neighbour slots for the tensor-core path (of_graph_multi_index); n_multi = number of such slots."""
-    __slots__ = ('tab', 'extra', 'taps', 'rows', 'tab_ord', 'multi_off', 'multi_types', 'n_multi', '_type_blocks', '_scan')
+    tab/extra: record encoding (CUDA-core path).  tab_ord/multi_off: ordinal encoding of the multi-neighbour slots for
+    the tensor-core path (of_graph_multi_index); n_multi = number of such slots."""
+    __slots__ = ('tab', 'extra', 'taps', 'rows', 'tab_ord', 'multi_off', 'n_multi', '_type_blocks', '_scan')
 
     def __init__(self, tab: torch.Tensor, extra, taps: int):
         assert tab.dtype == torch.int32 and tab.is_contiguous()
         self.tab, self.extra, self.taps = tab, extra, taps
         self.rows = tab.numel() // taps
-        self.tab_ord, self.multi_off, self.multi_types, self.n_multi = tab, None, None, 0
+        self.tab_ord, self.multi_off, self.n_multi = tab, None, 0
         self._type_blocks = {}
         self._scan = None
 
@@ -66,11 +65,6 @@ class TapTable:
             self._type_blocks[ntype] = out
         return self._type_blocks[ntype]
 
-    def index_multi(self, node_type=None):
-        """build the ordinal-encoded table (once per graph)."""
-        cnt = self.multi_prepare()
-        return self.multi_finish(int(cnt.item()), node_type)
-
     def multi_prepare(self):
         """flag + scan of the multi-neighbour slots; returns their count as a device scalar (no synchronisation)"""
         slots = self.tab.numel()
@@ -79,20 +73,17 @@ class TapTable:
         self._scan = exclusive_scan_i32(flags)
         return self._scan[-1:]
 
-    def multi_finish(self, n_multi: int, node_type=None):
-        slots = self.tab.numel()
-        dev = self.tab.device
+    def multi_finish(self, n_multi: int):
+        """build the ordinal-encoded table (once per graph) from multi_prepare's scan and its count"""
         scan = self._scan
         self._scan = None
         self.n_multi = int(n_multi)
         if self.n_multi == 0:
             return self
         self.tab_ord = torch.empty_like(self.tab)
-        self.multi_off = torch.empty(self.n_multi, dtype=torch.int32, device=dev)
-        self.multi_types = torch.empty(self.n_multi, dtype=torch.int64, device=dev)
-        check(lib.of_graph_multi_index(ptr(self.tab), ptr(self.extra), ptr(node_type) if node_type is not None else None,
-                                       slots, ptr(scan), ptr(self.tab_ord), ptr(self.multi_off),
-                                       ptr(self.multi_types), stream()), 'of_graph_multi_index')
+        self.multi_off = torch.empty(self.n_multi, dtype=torch.int32, device=self.tab.device)
+        check(lib.of_graph_multi_index(ptr(self.tab), ptr(self.extra), self.tab.numel(), ptr(scan), ptr(self.tab_ord),
+                                       ptr(self.multi_off), stream()), 'of_graph_multi_index')
         return self
 
 
@@ -183,13 +174,6 @@ class Stats:
         self.part, self.plan, self.channels, self.gran = part, plan, channels, gran
 
 
-_FUSE_STATS = os.environ.get('OCTFUSION_GN_FUSE', '1') != '0'     # 0: always run the stand-alone statistics pass
-# split-K for small-M tensor-core GEMMs (of_gather_gemm_tc_splitk): opt-in.  It sums K in another order than the
-# single-pass kernel, so its results differ in the last bits; the default keeps the single-pass kernel with the small-M
-# tile dispatch.  Its effect on the step time was not measured on H100.
-_SPLIT_K = os.environ.get('OCTFUSION_TC_SPLITK', '0') == '1'
-
-
 class PreparedWeight:
     """A GEMM weight in the two layouts the kernels read:
     canonical fp32 [taps*(c+ntype), N] (CUDA-core path) and the bf16 swizzled tile image (tensor-core
@@ -246,8 +230,8 @@ class PreparedWeight:
 
 
 def gather_gemm(a0, w: PreparedWeight, *, a1=None, tap: TapTable = None, in_rows=None, node_type=None,
-                a_silu=False, bias=None, row_add=None, row_add_idx=None, resid=None, out_rows=None,
-                out=None, ldo=None, out_f32=False, m=None, force_simt=False, stats: StatPlan = None):
+                bias=None, row_add=None, row_add_idx=None, resid=None, out_rows=None,
+                out=None, ldo=None, out_f32=False, stats: StatPlan = None):
     """out[m,:] = sum_tap mean_nbr [a0|a1|onehot] . W[tap] + bias + row_add[row_add_idx[m]] + resid[m].
     stats: the StatPlan of the output rows when a group norm consumes the output next -- the tensor-core epilogue then
     writes the norm's partial statistics (attached to the result as `_of_stats`), and ops.group_norm skips its
@@ -261,8 +245,7 @@ def gather_gemm(a0, w: PreparedWeight, *, a1=None, tap: TapTable = None, in_rows
         assert a1.dtype == a0.dtype and a1.stride(1) == 1
     taps = 1 if tap is None else tap.taps
     assert taps == w.taps
-    if m is None:
-        m = tap.rows if tap is not None else (in_rows.numel() if in_rows is not None else a0.shape[0])
+    m = tap.rows if tap is not None else (in_rows.numel() if in_rows is not None else a0.shape[0])
     n = w.n
     act_dtype = a0.dtype
     if out is None:
@@ -273,13 +256,12 @@ def gather_gemm(a0, w: PreparedWeight, *, a1=None, tap: TapTable = None, in_rows
         assert resid.dtype == act_dtype and resid.stride(1) == 1
     if w.ntype > 0:
         assert node_type is not None and node_type.dtype == torch.uint8
-    use_tc = (not _FORCE_SIMT and not force_simt and act_dtype == torch.bfloat16 and w.tc_ok() and c0 % 64 == 0
-              and c1 % 64 == 0 and not a_silu and m >= 1)
+    use_tc = (not _FORCE_SIMT and act_dtype == torch.bfloat16 and w.tc_ok() and c0 % 64 == 0 and c1 % 64 == 0
+              and m >= 1)
     g = GemmArgs()
     g.a0, g.lda0, g.c0 = a0.data_ptr(), a0.stride(0), c0
     g.a1, g.lda1, g.c1 = (a1.data_ptr(), a1.stride(0), c1) if a1 is not None else (None, 0, 0)
-    g.a_multi, g.ld_multi, g.multi_types = None, 0, None
-    g.rows_a0, g.rows_a1 = a0.shape[0], (a1.shape[0] if a1 is not None else 0)
+    g.a_multi, g.ld_multi = None, 0
     g.nt_block = None
     g.reverse = _next_direction() if use_tc else 0
     if use_tc and w.ntype > 0 and tap is not None:
@@ -292,7 +274,7 @@ def gather_gemm(a0, w: PreparedWeight, *, a1=None, tap: TapTable = None, in_rows
             check(lib.of_gather_mean_rows(a0.data_ptr(), a0.stride(0), c0, a1.data_ptr() if a1 is not None else None,
                                           a1.stride(0) if a1 is not None else 0, c1, ptr(tap.extra), ptr(tap.multi_off),
                                           tap.n_multi, dt(a0), ptr(aux), aux.stride(0), stream()), 'of_gather_mean_rows')
-            g.a_multi, g.ld_multi, g.multi_types = aux.data_ptr(), aux.stride(0), tap.multi_types.data_ptr()
+            g.a_multi, g.ld_multi = aux.data_ptr(), aux.stride(0)
     else:
         g.tap_tab = tap.tab.data_ptr() if tap is not None else None
     g.tap_extra = tap.extra.data_ptr() if (tap is not None and tap.extra is not None) else None
@@ -300,7 +282,6 @@ def gather_gemm(a0, w: PreparedWeight, *, a1=None, tap: TapTable = None, in_rows
     g.taps = taps
     g.node_type = node_type.data_ptr() if (node_type is not None and w.ntype > 0) else None
     g.ntype = w.ntype
-    g.a_silu = 1 if a_silu else 0
     g.w = (w.packed() if use_tc else w.canon).data_ptr()
     g.bias = bias.data_ptr() if bias is not None else None
     if row_add is not None:
@@ -316,7 +297,7 @@ def gather_gemm(a0, w: PreparedWeight, *, a1=None, tap: TapTable = None, in_rows
     g.dtype = dt(a0)
     st_obj = None
     g.stat_out, g.stat_chunk_seg, g.stat_seg_slot, g.stat_sample, g.stat_rows_per_sample = None, None, None, None, 0
-    if (stats is not None and _FUSE_STATS and use_tc and n % 32 == 0 and out_rows is None and stats.rows == m
+    if (stats is not None and use_tc and n % 32 == 0 and out_rows is None and stats.rows == m
             and not g.out_f32):
         st_obj = Stats(stats.new_part(n, tc_stat_gran(n)), stats, n, tc_stat_gran(n))
         g.stat_out, g.stat_chunk_seg = st_obj.part.data_ptr(), stats.chunk_seg.data_ptr()
@@ -328,13 +309,7 @@ def gather_gemm(a0, w: PreparedWeight, *, a1=None, tap: TapTable = None, in_rows
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record()
     if use_tc:
-        # launches whose row tiles cannot fill the GPU (the dense 4^3 level: 2048 rows, K up to 13824) split K over CTAs
-        splits = lib.of_tc_splitk_plan(C.byref(g)) if _SPLIT_K else 1
-        if splits > 1:
-            ws = torch.empty((splits, m, n), dtype=torch.float32, device=a0.device)
-            check(lib.of_gather_gemm_tc_splitk(C.byref(g), splits, ptr(ws), stream()), 'of_gather_gemm_tc_splitk')
-        else:
-            check(lib.of_gather_gemm_tc(C.byref(g), stream()), 'of_gather_gemm_tc')
+        check(lib.of_gather_gemm_tc(C.byref(g), stream()), 'of_gather_gemm_tc')
     else:
         check(lib.of_gather_gemm_simt(C.byref(g), stream()), 'of_gather_gemm_simt')
     if prof is not None:
@@ -367,19 +342,13 @@ def linear_small(x, weight, bias=None, a_silu=False):
 
 
 _sweep = [0]          # traversal direction of the next streaming kernel (see include/octfusion_b200.h: `reverse`)
-_alternate = [os.environ.get('OCTFUSION_ALTERNATE', '1') != '0']
 
 
 def _next_direction() -> int:
     """Alternate the row traversal direction from one big kernel to the next, so that each kernel starts on the rows
     its producer wrote (or read) last -- the part of the tensor that is still resident in L2."""
-    if not _alternate[0]:
-        return 0
     _sweep[0] ^= 1
     return _sweep[0]
-
-
-_gn_general = 2 if os.environ.get('OCTFUSION_GN_GENERAL') == '1' else 0      # diagnostics: disable the uniform-chunk path
 
 
 _ACT = {False: 0, None: 0, True: 1, 'silu': 1, 'gelu': 2}
@@ -441,7 +410,7 @@ def group_norm(x0, gamma, beta, groups: int, plan: StatPlan, *, x1=None, eps=1e-
     a1 = (ptr(x1), x1.stride(0), c1) if x1 is not None else (None, 0, 0)
     check(lib.of_gn_apply(ptr(x0), x0.stride(0), c0, a1[0], a1[1], a1[2], ptr(plan.sample_id), plan.rows_per_sample, rows,
                           ptr(scale), ptr(shift), _ACT[act], dt(x0), ptr(out), out.stride(0),
-                          _next_direction() | _gn_general, stream()), 'of_gn_apply')
+                          _next_direction(), stream()), 'of_gn_apply')
     if _PROFILE is not None:
         es = 2 if x0.dtype == torch.bfloat16 else 4
         _PROFILE.append(dict(kind='gn', M=rows, N=c, bytes=float(2 * rows * c * es), flops=0.0))

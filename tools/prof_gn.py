@@ -1,5 +1,5 @@
 """Times of_gn_stats / of_gn_finalize / of_gn_apply alone at the full B=32 size: achieved GB/s against the HBM peak.
-usage: python tools/prof_gn.py ; env REPS, OCTFUSION_GN_CHUNK_KB"""
+usage: python tools/prof_gn.py ; env REPS"""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
