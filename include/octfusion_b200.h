@@ -318,6 +318,43 @@ int of_mpu_eval_grid(const of_octree_levels* oct, int32_t depth, int32_t batch_i
                      float bbmax, int64_t head, int64_t count, const float* reg, float* fval, void* stream);
 
 /* ------------------------------------------------------------------------------------------
+ * Octree build from point clouds: ocnn.octree.Octree.build_octree (third-party; the reference calls it at
+ * models/octfusion_model_vae.py:135-146 and models/octfusion_model_union.py:200-212), restated from ocnn-pytorch 2.2.x
+ * in SURVEY.md Appendix B -- parity is UNPINNED at the ocnn boundary.
+ *   xyz [npts, 3] fp32 in [-1, 1] (values outside wrap: the integer coordinate is masked to `depth` bits), normals
+ *   [npts, 3] fp32 or NULL; the points of shape b are rows shape_offsets[b] .. shape_offsets[b+1] (int64 [batch + 1]
+ *   on the device).  Cell of a point: trunc((p + 1) * 2^(depth-1)) & (2^depth - 1) per axis; key = Morton | b << 48.
+ *   Limits: 0 <= full_depth < depth <= 16, 1 <= batch < 1024, npts < 2^31, batch * 8^full_depth < 2^31.
+ * Sequence: of_octree_build_levels (keys, stable radix sort, node ranks of depths full_depth..depth) -> the caller
+ * reads level_counts (its one host synchronisation) and allocates -> of_octree_build_fill per depth ->
+ * of_octree_build_signal.  The scratch (of_octree_build_bytes) carries the sorted keys between the calls and must not
+ * be reused until the last of them has run.  Results are bit-reproducible and independent of the launch configuration.
+ * ------------------------------------------------------------------------------------------ */
+/* scratch bytes of one build (O(npts)); OF_E_ARG when the arguments are out of range */
+int64_t of_octree_build_bytes(int64_t npts, int32_t batch, int32_t depth, int32_t full_depth);
+/* level_counts [depth + 2] int32: [d] = number of non-empty (distinct) nodes at depth d for full_depth <= d <= depth,
+ * 0 below full_depth; [depth + 1] = 1 when shape_offsets are not a partition of 0..npts (then nothing else is valid) */
+int of_octree_build_levels(const float* xyz, const int64_t* shape_offsets, int64_t npts, int32_t batch, int32_t depth,
+                           int32_t full_depth, void* scratch, int32_t* level_counts, void* stream);
+/* depth d = full_depth: children_d [batch * 8^full_depth] = rank among the non-empty nodes, -1 elsewhere (keys_d may be
+ * NULL: the full layer's keys are the octree_grow_full ones).  full_depth < d <= depth: nnum_d = 8 * level_counts[d-1];
+ * keys_d [nnum_d] = the 8 children of every non-empty depth-(d-1) node in key order, children_d [nnum_d] = rank of the
+ * child among the non-empty depth-d nodes, -1 when no point falls into it. */
+int of_octree_build_fill(const void* scratch, int64_t npts, int32_t batch, int32_t depth, int32_t full_depth, int32_t d,
+                         int64_t nnum_d, int64_t* keys_d, int32_t* children_d, void* stream);
+/* per non-empty depth-`depth` node r (level_counts[depth] rows): points [r, 3] = mean of (p + 1) * 2^(depth-1) over its
+ * points, normals [r, 3] = F.normalize(sum of its normals, eps = 1e-12); fp32 sums in input order.  normals_in and
+ * normals are both NULL or both set. */
+int of_octree_build_signal(const void* scratch, int64_t npts, int32_t batch, int32_t depth, int32_t full_depth,
+                           const float* xyz, const float* normals_in, float* points, float* normals, void* stream);
+/* ocnn InputFeature('ND', nempty=False) written as depth-D graph rows (DualOctree.get_input_feature, reference
+ * dual_octree.py:343-360): rows [0, leaf_rows) are zero (the leaves of full_depth..D-1), row leaf_rows + j is
+ * [normals[r] | sum((frac(points[r]) - 0.5) * normals[r])] with r = children[j], zero where r < 0.
+ * out [leaf_rows + nnum, >= 4] of dtype OF_F32 / OF_BF16, columns 0..3 written. */
+int of_input_feature_nd(const float* points, const float* normals, const int32_t* children, int64_t nnum,
+                        int64_t leaf_rows, int32_t dtype, void* out, int64_t ldo, void* stream);
+
+/* ------------------------------------------------------------------------------------------
  * Point-cloud shape metrics (reference metrics/evaluation_metrics.py: MMD, COV and 1-NNA with Chamfer distance and
  * approximate EMD).  Clouds are contiguous fp32 [count, points, 3].  "All pairs" entries compute every (i, j) of
  * a [na] x b [nb] into row-major [na, nb] outputs without copying any cloud; an entry is bit-identical to the same

@@ -100,6 +100,11 @@ _PROTOS = {
     'of_mc_emit': (C.c_int, [_vp, _i32, _f32, _vp, _vp, _vp, _vp, _vp]),
     'of_mesh_bbox': (C.c_int, [_vp, _vp, _i32, _vp, _vp]),
     'of_surface_sample': (C.c_int, [_vp, _vp, _vp, _vp, _i32, _i32, C.c_uint64, _vp, _vp, _vp, _vp]),
+    'of_octree_build_bytes': (_i64, [_i64, _i32, _i32, _i32]),
+    'of_octree_build_levels': (C.c_int, [_vp, _vp, _i64, _i32, _i32, _i32, _vp, _vp, _vp]),
+    'of_octree_build_fill': (C.c_int, [_vp, _i64, _i32, _i32, _i32, _i32, _i64, _vp, _vp, _vp]),
+    'of_octree_build_signal': (C.c_int, [_vp, _i64, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp]),
+    'of_input_feature_nd': (C.c_int, [_vp, _vp, _vp, _i64, _i64, _i32, _vp, _i64, _vp]),
 }
 
 EMD_MAX_POINTS = 4096              # OF_EMD_MAX_POINTS

@@ -3,7 +3,7 @@
 Drop-in for reference models/networks/dualoctree_networks/dual_octree.py `DualOctree` +
 `post_processing_for_docnn()` as far as the U-Net reads it (SURVEY.md 8b): `.graph[d]['edge_idx' |
 'edge_dir' | 'node_type']`, `.batch_id(d)`, `.batch_size`, `.nnum`, `.lnum`, `.node_child(d)`,
-`.octree`, `.total_num`.  Internally the graph is a *tap table* (one int32 per (row, direction)
+`.octree`, `.total_num`, and `.get_input_feature()` for octrees built from points.  Internally the graph is a *tap table* (one int32 per (row, direction)
 slot, see include/octfusion_b200.h) which is what the tap-gather GEMM consumes; the reference-format
 sorted edge lists are materialised lazily, only if somebody asks for them.
 """
@@ -166,6 +166,14 @@ class DualOctree:
 
     def node_child(self, depth):
         return self.octree.children[depth]
+
+    def get_input_feature(self, all_leaf_nodes=True, dtype=torch.float32):
+        """reference dual_octree.py:343-360: the ND input feature of the octree's depth-D nodes (InputFeature('ND')),
+        preceded by zero rows for the leaves of full_depth..D-1 when `all_leaf_nodes` -- i.e. one row per row of the
+        depth-D graph, written by one kernel in `dtype` (float32 or bfloat16)."""
+        from .modules import input_feature_nd
+        leaf_rows = int(self.lnum[self.full_depth:self.depth].sum()) if all_leaf_nodes else 0
+        return input_feature_nd(self.octree, leaf_rows, dtype)
 
     def _expand_edges(self, d, g):
         p = self.plan[d]

@@ -9,10 +9,11 @@ names (a reference checkpoint loads with `load_state_dict`), and the same operat
 kernels of liboctfusion_b200.so; the octree growth (`octree_split` / `octree_grow`) and the dual-graph rebuild per
 depth stay on the device.
 
-The encoder half is constructed (so that checkpoints load strictly) and `octree_encoder_step` is implemented on
-caller-provided input features; building those features from point clouds (`doctree.get_input_feature`, ocnn
-`InputFeature`) is outside this path.  `decode_code(pos=...)` / `output['neural_mpu']` evaluate the decoded implicit
-function with `mpu.NeuralMPU` (csrc/mpu.cu).
+The encoder runs on the ND input features of an octree built from points (`Octree.build_octree`,
+`DualOctree.get_input_feature`, csrc/points.cu) in `extract_code` and `forward` (graph_vae.py:246-298), or on
+caller-provided features in `octree_encoder_step` / `encode_moments`.  Inference only: `forward`'s `kl_loss` is a value,
+not a training loss.  `decode_code(pos=...)` / `output['neural_mpu']` evaluate the decoded implicit function with
+`mpu.NeuralMPU` (csrc/mpu.cu).
 """
 from __future__ import annotations
 import torch
@@ -164,12 +165,33 @@ class GraphDownsample(nn.Module):
         return out
 
 
+class DiagonalGaussianDistribution:
+    """reference distributions.py:24-63: mean | logvar halves of the moments, logvar clamped to [-30, 20]; `sample`
+    draws its noise from the host default generator (as the reference does) and moves it to the device."""
+
+    def __init__(self, parameters):
+        self.parameters = parameters.float()
+        self.mean, self.logvar = torch.chunk(self.parameters, 2, dim=1)
+        self.logvar = torch.clamp(self.logvar, -30.0, 20.0)
+        self.std = torch.exp(0.5 * self.logvar)
+        self.var = torch.exp(self.logvar)
+
+    def sample(self):
+        return self.mean + self.std * torch.randn(self.mean.shape).to(device=self.parameters.device)
+
+    def kl(self):
+        return 0.5 * (torch.pow(self.mean, 2) + self.var - 1.0 - self.logvar)
+
+    def mode(self):
+        return self.mean
+
+
 # =================================================================================================
 # the network
 # =================================================================================================
 class GraphVAE(nn.Module):
-    """reference graph_vae.py:50-131 (constructor), :171-223 (octree_decoder), :226-244 (create_*_octree),
-    :300-324 (decode_code)."""
+    """reference graph_vae.py:50-131 (constructor), :132-170 (encoder), :171-223 (octree_decoder), :226-244
+    (create_*_octree), :246-298 (forward, extract_code), :300-324 (decode_code)."""
 
     def __init__(self, depth, channel_in, nout, full_depth=2, depth_stop=6, depth_out=8, use_checkpoint=False,
                  resblk_type='bottleneck', bottleneck=4, resblk_num=3, code_channel=3, embed_dim=3):
@@ -229,7 +251,10 @@ class GraphVAE(nn.Module):
             octree_out.depth += 1
         return octree_out
 
-    # ---- encoder on given input features (graph_vae.py:135-170) ---------------------------------
+    # ---- encoder (graph_vae.py:132-170) -----------------------------------------------------------
+    def _get_input_feature(self, doctree, dtype=torch.float32):
+        return doctree.get_input_feature(dtype=dtype)
+
     @torch.no_grad()
     def octree_encoder_step(self, data, doctree):
         convd = data
@@ -246,6 +271,44 @@ class GraphVAE(nn.Module):
     def encode_moments(self, data, doctree):
         """mean | logvar of the posterior (`KL_conv`, graph_vae.py:163-168); sampling is the caller's."""
         return self.KL_conv(self.octree_encoder_step(data, doctree))
+
+    @torch.no_grad()
+    def octree_encoder(self, octree, doctree, dtype=torch.float32):
+        """posterior of the octree built from points (graph_vae.py:158-165)."""
+        return DiagonalGaussianDistribution(self.encode_moments(self._get_input_feature(doctree, dtype), doctree))
+
+    @torch.no_grad()
+    def extract_code(self, octree_in, dtype=torch.float32):
+        """graph_vae.py:291-298: (one posterior sample [rows of the depth_stop graph, embed_dim] fp32, the input's
+        DualOctree).  `dtype` is the activation dtype of the encoder (float32 or bfloat16)."""
+        doctree_in = DualOctree(octree_in)
+        return self.octree_encoder(octree_in, doctree_in, dtype).sample(), doctree_in
+
+    @torch.no_grad()
+    def forward(self, octree_in, octree_out=None, pos=None, evaluate=False, dtype=torch.float32):
+        """graph_vae.py:246-289 (inference): encode `octree_in`, sample the posterior (twice when `evaluate`, decoding
+        with the second sample, as the reference does), decode -- growing the octree from the labels when `octree_out`
+        is None.  The `neural_mpu` closure evaluates at depth_stop (:286).  `dtype` is the activation dtype."""
+        doctree_in = DualOctree(octree_in)
+        update_octree = octree_out is None
+        if update_octree:
+            octree_out = self.create_child_octree(octree_in)
+        doctree_out = DualOctree(octree_out)
+        posterior = self.octree_encoder(octree_in, doctree_in, dtype)
+        z = posterior.sample()
+        if evaluate:
+            z = posterior.sample()
+        out = self.octree_decoder(z.to(dtype), doctree_out, update_octree)
+        output = {'logits': out[0], 'reg_voxs': out[1], 'octree_out': out[2],
+                  'kl_loss': posterior.kl().mean(), 'code_max': z.max(), 'code_min': z.min()}
+        if pos is not None:
+            output['mpus'] = self.neural_mpu(pos, out[1], out[2])
+
+        def _neural_mpu(pos):
+            return self.neural_mpu(pos, out[1], out[2])[self.depth_stop][0]
+        _neural_mpu.mpu_args = (self.neural_mpu, out[1], out[2], self.depth_stop)
+        output['neural_mpu'] = _neural_mpu
+        return output
 
     # ---- decoder ---------------------------------------------------------------------------------
     @torch.no_grad()

@@ -572,3 +572,37 @@ class LearnedSinusoidalPosEmb(nn.Module):
     @torch.no_grad()
     def forward(self, x):
         return ops.learned_sinusoidal(x, self.weights)
+
+
+# =================================================================================================
+# input features of the GraphVAE encoder (ocnn.modules.InputFeature, SURVEY.md Appendix B: parity UNPINNED)
+# =================================================================================================
+def input_feature_nd(octree, leaf_rows: int = 0, dtype=torch.float32):
+    """[leaf_rows zero rows | ND feature of every depth-`octree.depth` node] (csrc/points.cu of_input_feature_nd): the
+    feature is [normal | sum((frac(point) - 0.5) * normal)] of a non-empty node and zero for an empty one."""
+    from ._lib import lib, ptr, stream, check, dt
+    D = octree.depth
+    points, normals = octree.points[D], octree.normals[D]
+    if points is None or normals is None:
+        raise RuntimeError('InputFeature ND: the octree has no points / normals at depth %d (build it with '
+                           'Octree.build_octree from points with normals)' % D)
+    child = octree.children[D].contiguous()
+    nnum = int(octree.nnum[D])
+    out = torch.empty((leaf_rows + nnum, 4), dtype=dtype, device=child.device)
+    check(lib.of_input_feature_nd(ptr(points.contiguous()), ptr(normals.contiguous()), ptr(child), nnum, leaf_rows,
+                                  dt(out), ptr(out), 4, stream()), 'of_input_feature_nd')
+    return out
+
+
+class InputFeature:
+    """ocnn.modules.InputFeature(feature='ND', nempty=False): [nnum[depth], 4] at the octree's depth, zero rows for the
+    empty nodes (octree_pad).  Only the N and D letters are built."""
+
+    def __init__(self, feature: str = 'ND', nempty: bool = False):
+        if feature.upper() != 'ND' or nempty:
+            raise NotImplementedError("InputFeature: only feature='ND' with nempty=False is built (got %r, nempty=%s)"
+                                      % (feature, nempty))
+        self.feature, self.nempty = feature, nempty
+
+    def __call__(self, octree):
+        return input_feature_nd(octree)

@@ -49,10 +49,10 @@ class NeuralMPU:
 
     @torch.no_grad()
     def eval_grid(self, reg_voxs, octree_out, batch_idx: int, size: int, bbmin: float, bbmax: float, head: int, count: int,
-                  out: torch.Tensor):
-        """finest-depth SDF at points [head, head+count) of the size^3 sampling grid of shape `batch_idx`, written into
-        out[head:head+count] (of_mpu_eval_grid: coordinates are generated inside the kernel)."""
-        d = self.depth
+                  out: torch.Tensor, depth=None):
+        """SDF at depth `depth` (default: the finest) at points [head, head+count) of the size^3 sampling grid of shape
+        `batch_idx`, written into out[head:head+count] (of_mpu_eval_grid: coordinates are generated inside the kernel)."""
+        d = self.depth if depth is None else depth
         reg = reg_voxs[d].float().contiguous()
         lv, keep = _levels(octree_out, d)
         check(lib.of_mpu_eval_grid(C.byref(lv), d, batch_idx, size, float(bbmin), float(bbmax), head, count, ptr(reg),
@@ -71,8 +71,8 @@ def get_mgrid(size: int, dim: int = 3, device='cuda'):
 def calc_sdf(model, batch_size: int = 1, size: int = 256, max_batch: int = 64 ** 3, bbmin: float = -1.0, bbmax: float = 1.0):
     """Drop-in for reference utils/util_dualoctree.py:99-118: the SDF of `batch_size` shapes on a size^3 grid,
     [B, size, size, size] fp32 on the device, evaluated in chunks of `max_batch` points.  `model` maps [P, 4] points
-    (x, y, z, batch index) to SDF values.  When it is the `neural_mpu` closure of `GraphVAE.decode_code` (it carries
-    `.mpu_args`), the grid coordinates are generated inside the evaluation kernel; any other callable gets explicit
+    (x, y, z, batch index) to SDF values.  When it is the `neural_mpu` closure of `GraphVAE.decode_code` or
+    `GraphVAE.forward` (it carries `.mpu_args`: the NeuralMPU, reg_voxs, octree and optionally the depth), the grid coordinates are generated inside the evaluation kernel; any other callable gets explicit
     point tensors exactly as in the reference."""
     num = size ** 3
     args = getattr(model, 'mpu_args', None)
@@ -84,8 +84,9 @@ def calc_sdf(model, batch_size: int = 1, size: int = 256, max_batch: int = 64 **
         while head < num:
             tail = min(head + max_batch, num)
             if args is not None:
-                mpu, reg_voxs, octree_out = args
-                mpu.eval_grid(reg_voxs, octree_out, b, size, bbmin, bbmax, head, tail - head, sdfs[b])
+                mpu, reg_voxs, octree_out = args[:3]
+                mpu.eval_grid(reg_voxs, octree_out, b, size, bbmin, bbmax, head, tail - head, sdfs[b],
+                              depth=args[3] if len(args) > 3 else None)
             else:
                 if samples is None:
                     samples = get_mgrid(size, 3, dev) * ((bbmax - bbmin) / size) + bbmin

@@ -6,12 +6,58 @@ batch index from bit 48 (dual_octree.py:75).
 
 This is host-side setup that runs once per batch of shapes (SURVEY.md 8f-2 marks the stage-1 ->
 stage-2 handoff as a "next" row); the per-step hot path never touches it.
+
+`Points` / `merge_points` / `Octree.build_octree` restate ocnn-pytorch 2.2.x (SURVEY.md Appendix B; parity UNPINNED at
+the ocnn boundary): the way into the VAE's latent space (reference models/octfusion_model_vae.py:135-146,
+datasets/dualoctree_snet.py:31-45).  The build runs on the CUDA kernels of csrc/points.cu.
 """
 from __future__ import annotations
+import ctypes as C
 import torch
 
 BATCH_SHIFT = 48
 KEY_MASK = (1 << 48) - 1
+MAX_DEPTH = 16             # 48-bit Morton key
+MAX_BATCH = 1024           # batch bits 48..57
+
+
+class Points:
+    """ocnn.octree.Points subset: points [N, 3], normals [N, 3] or None, batch_id [N] int64 (shapes contiguous and in
+    order), batch_size."""
+
+    def __init__(self, points, normals=None, batch_id=None, batch_size: int = 1):
+        self.points, self.normals, self.batch_size = points, normals, batch_size
+        self.batch_id = batch_id if batch_id is not None else torch.zeros(
+            points.shape[0], dtype=torch.long, device=points.device)
+        self.device = points.device
+
+    def clip(self, min: float = -1.0, max: float = 1.0, esp: float = 0.01):
+        """keeps the points with every coordinate strictly inside (min + esp, max - esp), with their normals and
+        batch ids."""
+        mask = ((self.points > min + esp) & (self.points < max - esp)).all(1)
+        self.points = self.points[mask]
+        self.normals = self.normals[mask] if self.normals is not None else None
+        self.batch_id = self.batch_id[mask]
+
+    def cuda(self):
+        return self.to('cuda')
+
+    def to(self, device):
+        self.points = self.points.to(device)
+        self.normals = self.normals.to(device) if self.normals is not None else None
+        self.batch_id = self.batch_id.to(device)
+        self.device = self.points.device
+        return self
+
+
+def merge_points(points: list):
+    """ocnn.octree.merge_points: the shapes concatenated in order, batch ids 0..B-1."""
+    has_normals = all(p.normals is not None for p in points)
+    return Points(torch.cat([p.points for p in points]),
+                  torch.cat([p.normals for p in points]) if has_normals else None,
+                  torch.cat([torch.full((p.points.shape[0],), i, dtype=torch.long, device=p.points.device)
+                             for i, p in enumerate(points)]),
+                  len(points))
 
 
 def xyz2key(x, y, z, b=None, depth: int = 16):
@@ -45,6 +91,60 @@ class Octree:
         self.children = [None] * n
         self.nnum = torch.zeros(n, dtype=torch.long)           # host counters (no device sync to read)
         self.nnum_nempty = torch.zeros(n, dtype=torch.long)
+        self.points = [None] * n                               # build_octree: per non-empty node of `depth`
+        self.normals = [None] * n
+
+    def build_octree(self, point_cloud: Points):
+        """ocnn Octree.build_octree (SURVEY.md Appendix B, UNPINNED): the octree of depth `self.depth` of every shape of
+        `point_cloud` (batch ids 0..batch_size-1, each shape's points contiguous), full layers up to full_depth, plus
+        points[depth] / normals[depth] (mean scaled point, normalised normal sum) per non-empty depth-`depth` node.
+        csrc/points.cu; one host synchronisation (the node counts of all depths)."""
+        from ._lib import lib, ptr, stream, check, require_cuda
+        D, fd, B = self.depth, self.full_depth, self.batch_size
+        if not (0 <= fd < D <= MAX_DEPTH and 1 <= B < MAX_BATCH):
+            raise ValueError('build_octree: need 0 <= full_depth < depth <= %d and 1 <= batch_size < %d (got %d, %d, %d)'
+                             % (MAX_DEPTH, MAX_BATCH, fd, D, B))
+        xyz = point_cloud.points
+        require_cuda(xyz)
+        if xyz.dim() != 2 or xyz.shape[1] != 3:
+            raise ValueError('build_octree: points must be [N, 3]')
+        xyz = xyz.to(device=self.device, dtype=torch.float32).contiguous()
+        nrm = point_cloud.normals
+        if nrm is not None:
+            if nrm.shape != xyz.shape:
+                raise ValueError('build_octree: normals must be [N, 3] like the points')
+            nrm = nrm.to(device=self.device, dtype=torch.float32).contiguous()
+        n = xyz.shape[0]
+        bid = point_cloud.batch_id.to(self.device).reshape(-1).long()
+        offsets = torch.searchsorted(bid, torch.arange(B + 1, device=self.device))
+        unsorted = (bid[1:] < bid[:-1]).sum().view(1).int()
+        nbytes = int(lib.of_octree_build_bytes(n, B, D, fd))
+        if nbytes < 0:
+            check(nbytes, 'of_octree_build_bytes')
+        scratch = torch.empty(max(nbytes, 8), dtype=torch.uint8, device=self.device)
+        counts = torch.empty(D + 2, dtype=torch.int32, device=self.device)
+        check(lib.of_octree_build_levels(ptr(xyz), ptr(offsets), n, B, D, fd, ptr(scratch), ptr(counts), stream()),
+              'of_octree_build_levels')
+        got = torch.cat([counts, unsorted]).tolist()                         # the one host synchronisation
+        if got[D + 1] or got[D + 2]:
+            raise ValueError('build_octree: batch ids must be 0..batch_size-1 with each shape contiguous')
+        for d in range(fd + 1):
+            self.octree_grow_full(d)
+        for d in range(fd, D + 1):
+            nnum = B * 8 ** fd if d == fd else 8 * got[d - 1]
+            keys = torch.empty(nnum, dtype=torch.long, device=self.device) if d > fd else None
+            child = torch.empty(nnum, dtype=torch.int32, device=self.device)
+            check(lib.of_octree_build_fill(ptr(scratch), n, B, D, fd, d, nnum, ptr(keys), ptr(child), stream()),
+                  'of_octree_build_fill')
+            if keys is not None:
+                self.keys[d] = keys
+            self.children[d] = child
+            self.nnum[d], self.nnum_nempty[d] = nnum, got[d]
+        self.points[D] = torch.empty((got[D], 3), dtype=torch.float32, device=self.device)
+        self.normals[D] = torch.empty((got[D], 3), dtype=torch.float32, device=self.device) if nrm is not None else None
+        check(lib.of_octree_build_signal(ptr(scratch), n, B, D, fd, ptr(xyz), ptr(nrm), ptr(self.points[D]),
+                                         ptr(self.normals[D]), stream()), 'of_octree_build_signal')
+        return self
 
     # growth: same semantics as the ocnn calls in ldm_diffusion_util.py:318-325 / util_dualoctree.py:238-248
     def octree_grow_full(self, depth: int, update_neigh: bool = False):
@@ -89,6 +189,8 @@ class Octree:
         self.device = torch.device(device)
         self.keys = [k.to(self.device) if k is not None else None for k in self.keys]
         self.children = [c.to(self.device) if c is not None else None for c in self.children]
+        self.points = [p.to(self.device) if p is not None else None for p in self.points]
+        self.normals = [p.to(self.device) if p is not None else None for p in self.normals]
         return self
 
     def cuda(self):

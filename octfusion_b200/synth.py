@@ -82,3 +82,20 @@ def synth_point_clouds(n: int, points: int, seed: int) -> torch.Tensor:
     centre = 0.45 + 0.1 * torch.rand(n, 1, 3, generator=g)
     radial = 1.0 + 0.01 * torch.randn(n, points, 1, generator=g)
     return (centre + direction * axes * radial).float().contiguous()
+
+
+def synth_shell_points(batch_size: int, points: int, seed: int = 0):
+    """per shape (xyz [points, 3], normals [points, 3]) fp32: points on a random ellipsoid shell inside (-1, 1)^3
+    (centre within 0.15 of the origin, semi-axes 0.21 .. 0.77) with the analytic unit normals -- the input of
+    Octree.build_octree in the encoder tests and benchmarks (a ShapeNet point cloud with normals has this form)."""
+    g = torch.Generator().manual_seed(seed)
+    out = []
+    for _ in range(batch_size):
+        u = torch.rand(7, generator=g, dtype=torch.float64)
+        centre = (u[0:3] * 2 - 1) * 0.15
+        axes = (0.6 + 0.8 * u[4:7]) * (0.35 + 0.20 * u[3])
+        d = torch.randn(points, 3, generator=g, dtype=torch.float64)
+        d = d / d.norm(dim=1, keepdim=True)
+        nrm = d / axes
+        out.append(((centre + d * axes).float(), (nrm / nrm.norm(dim=1, keepdim=True)).float()))
+    return out
