@@ -417,6 +417,39 @@ int of_surface_sample(const float* verts, const int64_t* vert_offsets, const int
                       int32_t batch, int32_t count, uint64_t seed, double* area_scan, float* points,
                       int32_t* face_index, void* stream);
 
+/* ------------------------------------------------------------------------------------------
+ * Mesh connected components and the largest-component filter of export_mesh(clean=True)
+ * (models/octfusion_model_union.py:459-466, models/octfusion_model_vae.py:242-250: trimesh split(only_watertight=False),
+ * then the component with the largest vertex bounding-box extent).  Rules restated from trimesh in DESIGN.md §4.6 --
+ * parity is UNPINNED at the trimesh boundary.  One shape per call: verts [nverts, 3] fp32, faces [nfaces, 3] int32 with
+ * shape-local ids.
+ *   weld       vertices with bit-identical (x, y, z) are one vertex, represented by the smallest id among them
+ *   adjacency  the edges (v0,v1), (v1,v2), (v2,v0) of every face on welded ids, unordered; an edge occurring exactly
+ *              twice in the shape links its two faces (once, or three times and more: no link)
+ *   labels     int32 [nfaces]: the smallest face index of the face's component (isolated faces are their own)
+ *   selection  extent = max over axes of (max - min) of the vertices the component's faces reference, in fp64 from the
+ *              fp32 coordinates; the largest extent is kept, the smaller label on a tie
+ *   output     the kept faces in their original order; their welded vertices in ascending id, renumbered from 0
+ * Sequence: of_mesh_components -> of_mesh_largest_component (same scratch, nothing in between) -> the caller reads the
+ * sizes in info (its one host synchronisation) and allocates -> of_mesh_compact.  Only integer atomics are used: the
+ * results are bit-reproducible and do not depend on the launch configuration.
+ * ------------------------------------------------------------------------------------------ */
+/* scratch bytes of one shape (O(nverts + nfaces), monotone in both); OF_E_ARG unless 0 <= nverts, nfaces < 2^31 */
+int64_t of_mesh_components_bytes(int64_t nverts, int64_t nfaces);
+/* labels [nfaces] as above.  info int32 [5]: [0] status, bit 0 = a coordinate is not finite, bit 1 = a face id lies
+ * outside [0, nverts) (no result is valid when status != 0); [1] number of components. */
+int of_mesh_components(const float* verts, int32_t nverts, const int32_t* faces, int32_t nfaces, void* scratch,
+                       int32_t* labels, int32_t* info, void* stream);
+/* after of_mesh_components on the same shape and scratch: info [2] kept label (-1 without faces), [3] kept faces,
+ * [4] kept vertices; vert_map [nverts] = output id of the vertex (every vertex welded to a kept one), -1 otherwise */
+int of_mesh_largest_component(const float* verts, int32_t nverts, const int32_t* faces, int32_t nfaces, void* scratch,
+                              const int32_t* labels, int32_t* vert_map, int32_t* info, void* stream);
+/* out_faces [info[3], 3] = vert_map of the faces with labels == label, in order; out_verts [info[4], 3] = the vertex
+ * each id came from.  Needs nverts, nfaces > 0; scratch as above (only its scan area is used). */
+int of_mesh_compact(const float* verts, int32_t nverts, const int32_t* faces, int32_t nfaces, const int32_t* labels,
+                    int32_t label, const int32_t* vert_map, void* scratch, float* out_verts, int32_t* out_faces,
+                    void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -105,6 +105,10 @@ _PROTOS = {
     'of_octree_build_fill': (C.c_int, [_vp, _i64, _i32, _i32, _i32, _i32, _i64, _vp, _vp, _vp]),
     'of_octree_build_signal': (C.c_int, [_vp, _i64, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp]),
     'of_input_feature_nd': (C.c_int, [_vp, _vp, _vp, _i64, _i64, _i32, _vp, _i64, _vp]),
+    'of_mesh_components_bytes': (_i64, [_i64, _i64]),
+    'of_mesh_components': (C.c_int, [_vp, _i32, _vp, _i32, _vp, _vp, _vp, _vp]),
+    'of_mesh_largest_component': (C.c_int, [_vp, _i32, _vp, _i32, _vp, _vp, _vp, _vp, _vp]),
+    'of_mesh_compact': (C.c_int, [_vp, _i32, _vp, _i32, _vp, _i32, _vp, _vp, _vp, _vp, _vp]),
 }
 
 EMD_MAX_POINTS = 4096              # OF_EMD_MAX_POINTS

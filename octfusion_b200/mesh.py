@@ -6,7 +6,9 @@ clouds) without leaving the device.  Replaces, in the reference,
       (models/octfusion_model_union.py:435-468)            -> marching_cubes(...).mesh(b), to_world(...)
   scale_to_unit_cube + trimesh mesh.sample(2048)
       (metrics/generate_pointclouds.py:14-37)               -> pointclouds_from_sdfs(...)
-The kernels are in csrc/mesh.cu; conventions (inside is f < level, vertex and face order, winding) are stated in
+  trimesh split(only_watertight=False) + the largest-extent pick of export_mesh(clean=True)
+      (models/octfusion_model_union.py:459-466)             -> connected_components(...), keep_largest_component(...)
+The kernels are in csrc/mesh.cu and csrc/mesh_components.cu; conventions (inside is f < level, vertex and face order, winding) are stated in
 include/octfusion_b200.h.  Inputs must be CUDA tensors: there is no CPU path.
 """
 from __future__ import annotations
@@ -15,7 +17,8 @@ import torch
 
 from ._lib import lib, ptr, stream, check, require_cuda, MC_MAX_SIZE
 
-__all__ = ['MeshBatch', 'marching_cubes', 'to_world', 'sample_surface', 'pointclouds_from_sdfs']
+__all__ = ['MeshBatch', 'marching_cubes', 'to_world', 'sample_surface', 'pointclouds_from_sdfs', 'connected_components',
+           'keep_largest_component']
 
 
 class MeshBatch:
@@ -153,15 +156,19 @@ def sample_surface(meshes: MeshBatch, count: int, seed: int = 0):
 
 
 @torch.no_grad()
-def pointclouds_from_sdfs(sdfs, n: int = 2048, level=0.0, seed: int = 0):
+def pointclouds_from_sdfs(sdfs, n: int = 2048, level=0.0, seed: int = 0, clean: bool = False):
     """[B, n, 3] fp32 metric point clouds of [B, R, R, R] SDF grids: marching_cubes, sample_surface, then
     scale_to_unit_cube (metrics/generate_pointclouds.py:14-21, padding 0: centre of the vertex bounding box to the
     origin, largest extent to 2) applied to the samples.  The normalisation removes any a * v + b map with a > 0, so
-    the to_world step of export_mesh is not needed here.  Feeds metrics.compute_all_metrics directly."""
+    the to_world step of export_mesh is not needed here.  clean=True keeps only the largest component of each mesh
+    (keep_largest_component, the clean=True step of export_mesh) before sampling.  Feeds
+    metrics.compute_all_metrics directly."""
     meshes = marching_cubes(sdfs, level)
     empty = _empty_shapes(meshes)
     if empty:
         raise ValueError('octfusion_b200.mesh: shapes %s have an empty mesh at level %g' % (empty, float(level)))
+    if clean:
+        meshes = keep_largest_component(meshes)
     points, _ = sample_surface(meshes, n, seed)
     B, dev = len(meshes), points.device
     with torch.cuda.device(dev):
@@ -170,3 +177,90 @@ def pointclouds_from_sdfs(sdfs, n: int = 2048, level=0.0, seed: int = 0):
     lo, hi = bbox[:, :3], bbox[:, 3:]
     scale = 2.0 / (hi - lo).amax(1)
     return ((points - ((lo + hi) * 0.5)[:, None]) * scale[:, None, None]).contiguous()
+
+
+def _component_inputs(meshes, what):
+    """(verts, faces, per-shape (V_b, F_b), scratch bytes) of a MeshBatch, checked"""
+    if not isinstance(meshes, MeshBatch):
+        raise TypeError('octfusion_b200.mesh: %s takes a MeshBatch' % what)
+    verts, faces = meshes.verts, meshes.faces
+    require_cuda(verts, faces)
+    if verts.dtype != torch.float32 or faces.dtype != torch.int32:
+        raise TypeError('octfusion_b200.mesh: %s needs float32 verts and int32 faces, got %s and %s'
+                        % (what, verts.dtype, faces.dtype))
+    if verts.dim() != 2 or verts.shape[1] != 3 or faces.dim() != 2 or faces.shape[1] != 3:
+        raise ValueError('octfusion_b200.mesh: %s needs verts [V, 3] and faces [F, 3], got %s and %s'
+                         % (what, tuple(verts.shape), tuple(faces.shape)))
+    if faces.device != verts.device:
+        raise ValueError('octfusion_b200.mesh: verts and faces are on different devices')
+    sizes = [(meshes._vo[b + 1] - meshes._vo[b], meshes._fo[b + 1] - meshes._fo[b]) for b in range(len(meshes))]
+    if any(nv < 0 or nf < 0 or nv >= 2 ** 31 or nf >= 2 ** 31 for nv, nf in sizes):
+        raise ValueError('octfusion_b200.mesh: every shape needs 0 <= vertex and face counts < 2^31')
+    nbytes = int(lib.of_mesh_components_bytes(max([nv for nv, _ in sizes], default=0),
+                                              max([nf for _, nf in sizes], default=0)))
+    return verts.contiguous(), faces.contiguous(), sizes, nbytes
+
+
+def _check_status(info):
+    nonfinite = [b for b, row in enumerate(info) if row[0] & 1]
+    if nonfinite:
+        raise ValueError('octfusion_b200.mesh: shapes %s have non-finite vertex coordinates' % nonfinite)
+    bad = [b for b, row in enumerate(info) if row[0] & 2]
+    if bad:
+        raise ValueError('octfusion_b200.mesh: shapes %s have faces with vertex ids outside the shape' % bad)
+
+
+def _components(meshes, what, largest):
+    """labels [F], info [B, 5] read to the host (the one synchronisation), and vert_map [V] when `largest`"""
+    verts, faces, sizes, nbytes = _component_inputs(meshes, what)
+    dev = verts.device
+    with torch.cuda.device(dev):
+        st = stream()
+        labels = torch.empty(faces.shape[0], dtype=torch.int32, device=dev)
+        vert_map = torch.empty(verts.shape[0], dtype=torch.int32, device=dev) if largest else None
+        info = torch.empty(len(meshes), 5, dtype=torch.int32, device=dev)
+        scratch = torch.empty(nbytes, dtype=torch.uint8, device=dev)     # sized by the largest shape, reused
+        for b, (nv, nf) in enumerate(sizes):
+            v, f, lab = _at(verts, meshes._vo[b]), _at(faces, meshes._fo[b]), _at(labels, meshes._fo[b])
+            check(lib.of_mesh_components(v, nv, f, nf, ptr(scratch), lab, _at(info, b), st), 'of_mesh_components')
+            if largest:
+                check(lib.of_mesh_largest_component(v, nv, f, nf, ptr(scratch), lab, _at(vert_map, meshes._vo[b]),
+                                                    _at(info, b), st), 'of_mesh_largest_component')
+        host = info.cpu().tolist()
+    _check_status(host)
+    return verts, faces, sizes, labels, vert_map, info, host, scratch
+
+
+@torch.no_grad()
+def connected_components(meshes: MeshBatch):
+    """(labels [F] int32, counts [B] int64), both on the device: the partition of trimesh `split(only_watertight=False)`
+    of every mesh.  Vertices with bit-identical coordinates are welded; two faces are adjacent when they share an
+    edge that occurs in exactly two faces of the shape.  labels[f] is the smallest shape-local face index of f's
+    component; counts[b] is the number of components of shape b.  One host synchronisation per call."""
+    _, _, _, labels, _, info, _, _ = _components(meshes, 'connected_components', False)
+    return labels, info[:, 1].to(torch.int64)
+
+
+@torch.no_grad()
+def keep_largest_component(meshes: MeshBatch) -> MeshBatch:
+    """The clean=True step of export_mesh (models/octfusion_model_union.py:459-466) on every mesh: the component (as in
+    connected_components) whose referenced vertices have the largest bounding-box extent, max over axes of
+    (max - min) in fp64; on a tie the one with the smaller label.  Its faces keep their order; its welded vertices
+    keep ascending id order, renumbered from 0.  An empty shape stays empty.  One host synchronisation per call."""
+    verts, faces, sizes, labels, vert_map, _, host, scratch = _components(meshes, 'keep_largest_component', True)
+    dev = verts.device
+    vo, fo = [0], [0]
+    for row in host:
+        vo.append(vo[-1] + row[4])
+        fo.append(fo[-1] + row[3])
+    with torch.cuda.device(dev):
+        st = stream()
+        out_v = torch.empty(vo[-1], 3, dtype=torch.float32, device=dev)
+        out_f = torch.empty(fo[-1], 3, dtype=torch.int32, device=dev)
+        for b, (nv, nf) in enumerate(sizes):
+            if host[b][3] == 0:
+                continue
+            check(lib.of_mesh_compact(_at(verts, meshes._vo[b]), nv, _at(faces, meshes._fo[b]), nf,
+                                      _at(labels, meshes._fo[b]), host[b][2], _at(vert_map, meshes._vo[b]),
+                                      ptr(scratch), _at(out_v, vo[b]), _at(out_f, fo[b]), st), 'of_mesh_compact')
+    return MeshBatch(out_v, out_f, vo, fo)
