@@ -60,10 +60,13 @@ int of_abi_sizeof_octree_levels(void);
  *   the "+ emb_out[batch_id]" loop    modules.py:757-758   (row_add)
  *   the residual / skip add           modules.py:513, 763  (resid)
  *
- * Neighbour table `tap_tab` [M, taps] int32 (row-major):
+ * Neighbour table `tap_tab` [M, taps] int32 (row-major), the one encoding every reader uses:
  *      v >= 0 : exactly one source row v
  *      v == -1: no neighbour (slot contributes zero; count clamps to 1, scatter.py:60)
- *      v <= -2: several sources: o = -(v+2); tap_extra[o] = count n, tap_extra[o+1..o+n] = rows
+ *      v <= -2: several sources: multi-neighbour slot o = -(v+2), 0 <= o < n_multi, numbered in slot order
+ *   `tap_extra` int32 [n_multi + 1 + words] lists the sources of the multi slots in CSR form: tap_extra[0..n_multi]
+ *   are offsets into tap_extra itself, and the rows of slot o are tap_extra[tap_extra[o] .. tap_extra[o+1]), in the
+ *   order of_graph_fill enumerates them.  May be NULL when the table has no multi slot.
  *   tap_tab == NULL: identity (taps must be 1); source row = in_rows ? in_rows[m] : m
  * A is the channel concatenation of up to two sources (a0 | a1) -- the torch.cat of the skip
  * stack (graph_unet_hr.py:266) is never materialised.
@@ -87,12 +90,11 @@ typedef struct of_gemm_args {
   int32_t out_f32;                               /* 1: write fp32 regardless of dtype         */
   int32_t M, N;
   int32_t dtype;                                 /* activation dtype of a0/a1/resid/out       */
-  /* tensor-core path only: slots with several neighbours read their pre-averaged row.  There tap_tab uses
-   * the ORDINAL encoding of of_graph_multi_index: v <= -2 -> row -(v+2) of a_multi (built per input tensor
+  /* tensor-core path only: multi slot o reads row o of a_multi, its pre-averaged sources (built per input tensor
    * by of_gather_mean_rows).                                                                                 */
   const void* a_multi; int64_t ld_multi;
   /* tensor-core path with ntype > 0 (required there): the node-type K block as a precomputed bf16 [M, 64] tensor
-   * (of_graph_type_block, record-encoded table)                                                              */
+   * (of_graph_type_block)                                                                                    */
   const void* nt_block;
   /* tensor-core path: 1 = walk the row tiles from the last to the first.  Alternating the direction from one kernel to
    * the next lets each kernel start on the rows its producer wrote last, which are still in the 50 MB L2.  */
@@ -220,8 +222,8 @@ int of_copy_rows(const void* src, int64_t lds, int32_t src_dtype, const int32_t*
  *
  * of_leaf_rank / of_compact_idx   per level: rank of every leaf among the leaves of its depth, and the
  *                 index lists of leaf / non-empty nodes (row maps of GraphDownsample / GraphUpsample)
- * of_graph_count  pass 1: need[row*7+dir] = words of tap_extra the slot needs (0 for <= 1 neighbour)
- * of_exclusive_scan_i32 over `need`
+ * of_graph_count  pass 1: per slot, the rows it lists in tap_extra and whether it is a multi slot
+ * of_exclusive_scan_i32 over both
  * of_graph_fill   pass 2: final tap_tab [rows, 7] (dir 6 = self loop, dual_octree.py:241-249) and
  *                 tap_extra; also node_type [rows] uint8 (:381-389) and batch_id [rows] int32 (:65-79)
  * ------------------------------------------------------------------------------------------ */
@@ -245,29 +247,25 @@ int of_compact_idx(const int32_t* children, const int32_t* leaf_rank, int32_t n,
                    int32_t* leaf_idx, int32_t* nonempty_idx, void* stream);
 /* number of rows of the depth-D graph (host arithmetic on nnum; no device work) */
 int64_t of_graph_rows(const of_octree_levels* oct, int32_t D);
-/* pass 1: need[row*7 + dir] = words of tap_extra the slot needs (0 when it has <= 1 neighbour) */
-int of_graph_count(const of_octree_levels* oct, int32_t D, int32_t* need, void* stream);
-/* pass 2: need_off = exclusive scan of need */
-int of_graph_fill(const of_octree_levels* oct, int32_t D, const int32_t* need_off,
-                  int32_t* tap_tab, int32_t* tap_extra, uint8_t* node_type, int32_t* batch_id,
+/* Multi-neighbour slots: a coarse leaf next to a subdivided cell, 4..16 finer neighbours averaged by scatter_mean
+ * (utils/scatter.py:42-66); up to 4^k for k adaptive levels.
+ * pass 1: need[row*7 + dir] = number of neighbours of a multi slot, else 0; multi[row*7 + dir] = 1 for a multi slot,
+ * else 0. */
+int of_graph_count(const of_octree_levels* oct, int32_t D, int32_t* need, int32_t* multi, void* stream);
+/* pass 2: need_off / multi_ord = exclusive scans of need / multi, n_multi = total of multi; tap_extra holds
+ * n_multi + 1 + (total of need) words. */
+int of_graph_fill(const of_octree_levels* oct, int32_t D, const int32_t* need_off, const int32_t* multi_ord,
+                  int32_t n_multi, int32_t* tap_tab, int32_t* tap_extra, uint8_t* node_type, int32_t* batch_id,
                   void* stream);
-/* Multi-neighbour slots (coarse leaf next to a subdivided cell: 4..16 finer neighbours, averaged by
- * scatter_mean, utils/scatter.py:42-66; up to 4^k for k adaptive levels).  of_graph_multi_flags marks them (flags[i] = tap_tab[i] <= -2);
- * after an exclusive scan of the flags, of_graph_multi_index writes the ordinal-encoded table used by the
- * tensor-core path (v <= -2 -> -(ordinal+2)) and multi_off[ord] = offset of the slot's record in tap_extra.
- * of_gather_mean_rows: out[ord, :] = mean over the slot's neighbours of (a0|a1)[row, :]  (per input tensor). */
-int of_graph_multi_flags(const int32_t* tap_tab, int64_t slots, int32_t* flags, void* stream);
-int of_graph_multi_index(const int32_t* tap_tab, const int32_t* tap_extra, int64_t slots, const int32_t* flag_scan,
-                         int32_t* tap_tab_ord, int32_t* multi_off, void* stream);
 /* Node-type K block of the tensor-core GEMM, a per-graph constant: out [rows, 64] bf16, column tap*ntype + type =
  * (#neighbours of that type in slot (row, tap)) / (#neighbours) = the scatter_mean of the one-hot columns that
  * GraphConv.forward appends to the features (models/networks/modules.py:199-202, 208-210); zero elsewhere.
- * tap_tab / tap_extra are the RECORD-encoded tables of of_graph_fill.  Requires taps*ntype <= 64, ntype <= 8. */
+ * Requires taps*ntype <= 64, ntype <= 8. */
 int of_graph_type_block(const int32_t* tap_tab, const int32_t* tap_extra, const uint8_t* node_type, int64_t rows,
                         int32_t taps, int32_t ntype, void* out_bf16, void* stream);
+/* out[o, :] = mean over the rows of multi slot o of (a0|a1)[row, :], o < count (once per input tensor) */
 int of_gather_mean_rows(const void* a0, int64_t lda0, int32_t c0, const void* a1, int64_t lda1, int32_t c1,
-                        const int32_t* tap_extra, const int32_t* multi_off, int32_t count, int32_t dtype,
-                        void* out, int64_t ldo, void* stream);
+                        const int32_t* tap_extra, int32_t count, int32_t dtype, void* out, int64_t ldo, void* stream);
 /* hist[v] += 1 for v = values[i] (caller zeroes hist) -- rows per sample for the norm count */
 int of_histogram_i32(const int32_t* values, int64_t n, int32_t bins, int32_t* hist, void* stream);
 /* reference-format edge list (edge_idx [2,E], edge_dir [E] int64, sorted by row*7+dir:

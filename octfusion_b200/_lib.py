@@ -79,13 +79,11 @@ _PROTOS = {
     'of_exclusive_scan_i32': (C.c_int, [_vp, _vp, _i64, _vp, _vp, _vp]),
     'of_compact_idx': (C.c_int, [_vp, _vp, _i32, _vp, _vp, _vp]),
     'of_graph_rows': (_i64, [C.POINTER(OctreeLevels), _i32]),
-    'of_graph_count': (C.c_int, [C.POINTER(OctreeLevels), _i32, _vp, _vp]),
-    'of_graph_fill': (C.c_int, [C.POINTER(OctreeLevels), _i32, _vp, _vp, _vp, _vp, _vp, _vp]),
+    'of_graph_count': (C.c_int, [C.POINTER(OctreeLevels), _i32, _vp, _vp, _vp]),
+    'of_graph_fill': (C.c_int, [C.POINTER(OctreeLevels), _i32, _vp, _vp, _i32, _vp, _vp, _vp, _vp, _vp]),
     'of_histogram_i32': (C.c_int, [_vp, _i64, _i32, _vp, _vp]),
-    'of_graph_multi_flags': (C.c_int, [_vp, _i64, _vp, _vp]),
-    'of_graph_multi_index': (C.c_int, [_vp, _vp, _i64, _vp, _vp, _vp, _vp]),
     'of_graph_type_block': (C.c_int, [_vp, _vp, _vp, _i64, _i32, _i32, _vp, _vp]),
-    'of_gather_mean_rows': (C.c_int, [_vp, _i64, _i32, _vp, _i64, _i32, _vp, _vp, _i32, _i32, _vp, _i64, _vp]),
+    'of_gather_mean_rows': (C.c_int, [_vp, _i64, _i32, _vp, _i64, _i32, _vp, _i32, _i32, _vp, _i64, _vp]),
     'of_graph_edge_count': (C.c_int, [_vp, _vp, _i64, _vp, _vp]),
     'of_graph_edges': (C.c_int, [_vp, _vp, _i64, _i32, _vp, _vp, _vp, _vp, _vp]),
     'of_dense_tap_table': (C.c_int, [_i32, _i32, _i32, _vp, _vp]),
@@ -122,7 +120,7 @@ class LibraryMissing(ImportError):
     pass
 
 
-ABI_VERSION = 6          # of_version() of the header this binding mirrors
+ABI_VERSION = 7          # of_version() of the header this binding mirrors
 
 
 def _load():

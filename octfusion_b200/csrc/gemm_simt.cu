@@ -30,10 +30,10 @@ __device__ __forceinline__ float load_a(const of_gemm_args& p, int m, int tap, i
   int t = p.tap_tab[(int64_t)m * p.taps + tap];
   if (t == -1) return 0.0f;
   if (t >= 0) return load_feat<T>(p, t, c);
-  const int32_t* e = p.tap_extra + (-(t + 2));
-  int n = e[0];
+  const int32_t* e = p.tap_extra + p.tap_extra[-(t + 2)];
+  const int n = p.tap_extra[-(t + 1)] - p.tap_extra[-(t + 2)];
   float s = 0.0f;
-  for (int i = 1; i <= n; ++i) s += load_feat<T>(p, e[i], c);
+  for (int i = 0; i < n; ++i) s += load_feat<T>(p, e[i], c);
   return s / (float)n;
 }
 

@@ -12,7 +12,8 @@
 // No hashing, no sort: rows come out in graph order and each (row, dir) slot is written once.
 //
 // Output is the tap table consumed by the tap-gather GEMM (include/octfusion_b200.h):
-// tab[row, 7] int32 with -1 / single row / -(offset+2) into tap_extra for 4..16 finer neighbours.
+// tab[row, 7] int32 with -1 / single row / -(o+2) for the o-th multi-neighbour slot, whose rows tap_extra lists in
+// CSR form.
 #include "common.cuh"
 
 namespace of {
@@ -224,7 +225,7 @@ __device__ __forceinline__ void for_each_face_neighbour(const GraphCtx& g, int d
   }
 }
 
-__global__ void graph_count_kernel(GraphCtx g, int d, int32_t* __restrict__ need) {
+__global__ void graph_count_kernel(GraphCtx g, int d, int32_t* __restrict__ need, int32_t* __restrict__ multi) {
   const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   const int i = (int)(idx / 6), dir = (int)(idx % 6);
   if (i >= g.nnum[d]) return;
@@ -234,11 +235,16 @@ __global__ void graph_count_kernel(GraphCtx g, int d, int32_t* __restrict__ need
   int n = 0;
   for_each_face_neighbour(g, d, x, y, z, b, dir, [&](int) { ++n; });
   const int64_t row = graph_row(g, d, i);
-  need[row * 7 + dir] = n > 1 ? n + 1 : 0;
-  if (dir == 0) need[row * 7 + 6] = 0;
+  need[row * 7 + dir] = n > 1 ? n : 0;
+  multi[row * 7 + dir] = n > 1 ? 1 : 0;
+  if (dir == 0) need[row * 7 + 6] = multi[row * 7 + 6] = 0;
 }
 
-__global__ void graph_fill_kernel(GraphCtx g, int d, const int32_t* __restrict__ need_off, int32_t* __restrict__ tab,
+// need_off / multi_ord: exclusive scans of of_graph_count's need / multi.  The rows of multi slot o start at word
+// n_multi + 1 + need_off[slot] of extra; the thread of row 0 writes the closing offset, so that it exists even when the
+// graph has no multi slot.
+__global__ void graph_fill_kernel(GraphCtx g, int d, const int32_t* __restrict__ need_off,
+                                  const int32_t* __restrict__ multi_ord, int32_t n_multi, int32_t* __restrict__ tab,
                                   int32_t* __restrict__ extra, uint8_t* __restrict__ node_type,
                                   int32_t* __restrict__ batch_id) {
   const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -249,25 +255,27 @@ __global__ void graph_fill_kernel(GraphCtx g, int d, const int32_t* __restrict__
   key_decode(g.keys[d][i], d, x, y, z, b);
   const int64_t row = graph_row(g, d, i);
   const int64_t slot = row * 7 + dir;
-  const int32_t off = need_off[slot];
-  const int32_t cap = need_off[slot + 1] - off;
+  const int32_t off = n_multi + 1 + need_off[slot];
+  const int32_t cap = need_off[slot + 1] - need_off[slot];
   if (cap == 0) {
     int32_t v = -1;
     for_each_face_neighbour(g, d, x, y, z, b, dir, [&](int r) { v = r; });
     tab[slot] = v;
   } else {
+    const int32_t o = multi_ord[slot];
     int n = 0;
     for_each_face_neighbour(g, d, x, y, z, b, dir, [&](int r) {
-      if (n + 1 < cap) extra[off + 1 + n] = r;
+      if (n < cap) extra[off + n] = r;
       ++n;
     });
-    extra[off] = n;
-    tab[slot] = -(off + 2);
+    extra[o] = off;
+    tab[slot] = -(o + 2);
   }
   if (dir == 0) {
     tab[row * 7 + 6] = (int32_t)row;                       // self loop, dual_octree.py:241-249
     if (node_type) node_type[row] = (uint8_t)(d - g.fd);   // dual_octree.py:381-389
     if (batch_id) batch_id[row] = b;                       // dual_octree.py:65-79
+    if (row == 0) extra[n_multi] = n_multi + 1 + need_off[(int64_t)(g.row_base[g.D] + g.nnum[g.D]) * 7];
   }
 }
 
@@ -303,7 +311,7 @@ __global__ void edge_count_kernel(const int32_t* __restrict__ tab, const int32_t
   const int64_t s = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (s >= slots) return;
   const int t = tab[s];
-  per_slot[s] = t == -1 ? 0 : t >= 0 ? 1 : extra[-(t + 2)];
+  per_slot[s] = t == -1 ? 0 : t >= 0 ? 1 : extra[-(t + 1)] - extra[-(t + 2)];
 }
 
 __global__ void edge_fill_kernel(const int32_t* __restrict__ tab, const int32_t* __restrict__ extra, int64_t slots,
@@ -316,25 +324,7 @@ __global__ void edge_fill_kernel(const int32_t* __restrict__ tab, const int32_t*
   const int64_t row = s / taps, dir = s % taps;
   int64_t o = slot_off[s];
   if (t >= 0) { er[o] = row; ec[o] = t; ed[o] = dir; return; }
-  const int32_t* e = extra + (-(t + 2));
-  const int n = e[0];
-  for (int j = 1; j <= n; ++j, ++o) { er[o] = row; ec[o] = e[j]; ed[o] = dir; }
-}
-
-__global__ void multi_flags_kernel(const int32_t* __restrict__ tab, int64_t slots, int32_t* __restrict__ flags) {
-  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < slots) flags[i] = tab[i] <= -2 ? 1 : 0;
-}
-
-__global__ void multi_index_kernel(const int32_t* __restrict__ tab, int64_t slots, const int32_t* __restrict__ scan,
-                                   int32_t* __restrict__ tab_ord, int32_t* __restrict__ multi_off) {
-  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= slots) return;
-  const int32_t v = tab[i];
-  if (v > -2) { tab_ord[i] = v; return; }
-  const int32_t ord = scan[i];
-  tab_ord[i] = -(ord + 2);
-  multi_off[ord] = -(v + 2);
+  for (int j = extra[-(t + 2)], end = extra[-(t + 1)]; j < end; ++j, ++o) { er[o] = row; ec[o] = extra[j]; ed[o] = dir; }
 }
 
 // Node-type K block of the tensor-core GEMM, precomputed once per graph: row m, column tap*ntype + type holds
@@ -358,9 +348,9 @@ __global__ void type_block_kernel(const int32_t* __restrict__ tab, const int32_t
     if (tv >= 0) {
       cnt[node_type[tv] & 7] = 1;
     } else {
-      const int32_t* e = extra + (-(tv + 2));
-      n = e[0];
-      for (int k = 1; k <= n; ++k) ++cnt[node_type[e[k]] & 7];
+      const int32_t j0 = extra[-(tv + 2)], j1 = extra[-(tv + 1)];
+      n = j1 - j0;
+      for (int j = j0; j < j1; ++j) ++cnt[node_type[extra[j]] & 7];
     }
 #pragma unroll
     for (int ty = 0; ty < 8; ++ty)
@@ -368,26 +358,25 @@ __global__ void type_block_kernel(const int32_t* __restrict__ tab, const int32_t
   }
 }
 
-// one thread per (slot, 16-byte chunk): mean over the slot's neighbours, fp32 accumulate
+// one thread per (multi slot, 16-byte chunk): mean over the slot's neighbours, fp32 accumulate
 template <typename T, int V>
 __global__ void gather_mean_rows_kernel(const T* __restrict__ a0, int64_t lda0, int c0, const T* __restrict__ a1,
-                                        int64_t lda1, int c1, const int32_t* __restrict__ extra,
-                                        const int32_t* __restrict__ multi_off, int count, T* __restrict__ out,
-                                        int64_t ldo) {
+                                        int64_t lda1, int c1, const int32_t* __restrict__ extra, int count,
+                                        T* __restrict__ out, int64_t ldo) {
   const int cpr = (c0 + c1) / V;
   const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= (int64_t)count * cpr) return;
   const int ord = (int)(idx / cpr);
   const int c = (int)(idx - (int64_t)ord * cpr) * V;
-  const int32_t* e = extra + multi_off[ord];
-  const int n = e[0];
+  const int32_t j0 = extra[ord], j1 = extra[ord + 1];
+  const int n = j1 - j0;
   const T* base = c < c0 ? a0 + c : a1 + (c - c0);
   const int64_t ld = c < c0 ? lda0 : lda1;
   float acc[V];
 #pragma unroll
   for (int j = 0; j < V; ++j) acc[j] = 0.0f;
-  for (int k = 1; k <= n; ++k) {
-    const T* src = base + (int64_t)e[k] * ld;
+  for (int k = j0; k < j1; ++k) {
+    const T* src = base + (int64_t)extra[k] * ld;
     if (V == 8) {
       float f[8];
       bf16x8_to_f32(*reinterpret_cast<const uint4*>(src), f);
@@ -415,26 +404,6 @@ __global__ void gather_mean_rows_kernel(const T* __restrict__ a0, int64_t lda0, 
 
 using namespace of;
 
-extern "C" int of_graph_multi_flags(const int32_t* tap_tab, int64_t slots, int32_t* flags, void* stream) {
-  OF_REQUIRE(tap_tab && flags && slots >= 0, "of_graph_multi_flags: bad arguments");
-  if (slots == 0) return OF_OK;
-  multi_flags_kernel<<<(unsigned)((slots + 255) / 256), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(tap_tab, slots,
-                                                                                                        flags);
-  OF_LAUNCH_CHECK("of_graph_multi_flags");
-  return OF_OK;
-}
-
-extern "C" int of_graph_multi_index(const int32_t* tap_tab, const int32_t* tap_extra, int64_t slots,
-                                    const int32_t* flag_scan, int32_t* tap_tab_ord, int32_t* multi_off, void* stream) {
-  OF_REQUIRE(tap_tab && tap_extra && flag_scan && tap_tab_ord && multi_off && slots >= 0,
-             "of_graph_multi_index: bad arguments");
-  if (slots == 0) return OF_OK;
-  multi_index_kernel<<<(unsigned)((slots + 255) / 256), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
-      tap_tab, slots, flag_scan, tap_tab_ord, multi_off);
-  OF_LAUNCH_CHECK("of_graph_multi_index");
-  return OF_OK;
-}
-
 extern "C" int of_graph_type_block(const int32_t* tap_tab, const int32_t* tap_extra, const uint8_t* node_type, int64_t rows,
                                    int32_t taps, int32_t ntype, void* out_bf16, void* stream) {
   OF_REQUIRE(tap_tab && node_type && out_bf16 && rows >= 0 && taps > 0 && ntype > 0 && taps * ntype <= 64 && ntype <= 8,
@@ -447,9 +416,9 @@ extern "C" int of_graph_type_block(const int32_t* tap_tab, const int32_t* tap_ex
 }
 
 extern "C" int of_gather_mean_rows(const void* a0, int64_t lda0, int32_t c0, const void* a1, int64_t lda1, int32_t c1,
-                                   const int32_t* tap_extra, const int32_t* multi_off, int32_t count, int32_t dtype,
-                                   void* out, int64_t ldo, void* stream) {
-  OF_REQUIRE(a0 && c0 > 0 && ((a1 == nullptr) == (c1 == 0)) && tap_extra && multi_off && out && count >= 0,
+                                   const int32_t* tap_extra, int32_t count, int32_t dtype, void* out, int64_t ldo,
+                                   void* stream) {
+  OF_REQUIRE(a0 && c0 > 0 && ((a1 == nullptr) == (c1 == 0)) && tap_extra && out && count >= 0,
              "of_gather_mean_rows: bad arguments");
   OF_REQUIRE(dtype == OF_F32 || dtype == OF_BF16, "of_gather_mean_rows: bad dtype");
   if (count == 0) return OF_OK;
@@ -458,17 +427,17 @@ extern "C" int of_gather_mean_rows(const void* a0, int64_t lda0, int32_t c0, con
   if (dtype == OF_BF16 && c0 % 8 == 0 && c1 % 8 == 0 && lda0 % 8 == 0 && lda1 % 8 == 0 && ldo % 8 == 0) {
     const int64_t n = (int64_t)count * (C / 8);
     gather_mean_rows_kernel<__nv_bfloat16, 8><<<(unsigned)((n + 255) / 256), 256, 0, st>>>(
-        (const __nv_bfloat16*)a0, lda0, c0, (const __nv_bfloat16*)a1, lda1, c1, tap_extra, multi_off, count,
+        (const __nv_bfloat16*)a0, lda0, c0, (const __nv_bfloat16*)a1, lda1, c1, tap_extra, count,
         (__nv_bfloat16*)out, ldo);
   } else if (dtype == OF_BF16) {
     const int64_t n = (int64_t)count * C;
     gather_mean_rows_kernel<__nv_bfloat16, 1><<<(unsigned)((n + 255) / 256), 256, 0, st>>>(
-        (const __nv_bfloat16*)a0, lda0, c0, (const __nv_bfloat16*)a1, lda1, c1, tap_extra, multi_off, count,
+        (const __nv_bfloat16*)a0, lda0, c0, (const __nv_bfloat16*)a1, lda1, c1, tap_extra, count,
         (__nv_bfloat16*)out, ldo);
   } else {
     const int64_t n = (int64_t)count * C;
     gather_mean_rows_kernel<float, 1><<<(unsigned)((n + 255) / 256), 256, 0, st>>>(
-        (const float*)a0, lda0, c0, (const float*)a1, lda1, c1, tap_extra, multi_off, count, (float*)out, ldo);
+        (const float*)a0, lda0, c0, (const float*)a1, lda1, c1, tap_extra, count, (float*)out, ldo);
   }
   OF_LAUNCH_CHECK("of_gather_mean_rows");
   return OF_OK;
@@ -504,34 +473,35 @@ extern "C" int64_t of_graph_rows(const of_octree_levels* oct, int32_t D) {
   return (int64_t)g.row_base[D] + oct->nnum[D];
 }
 
-extern "C" int of_graph_count(const of_octree_levels* oct, int32_t D, int32_t* need, void* stream) {
+extern "C" int of_graph_count(const of_octree_levels* oct, int32_t D, int32_t* need, int32_t* multi, void* stream) {
   GraphCtx g;
   int rc = make_ctx(oct, D, g, "of_graph_count");
   if (rc) return rc;
-  OF_REQUIRE(need != nullptr, "of_graph_count: null output");
+  OF_REQUIRE(need && multi, "of_graph_count: null output");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   for (int d = g.fd; d <= D; ++d) {
     const int64_t n = (int64_t)g.nnum[d] * 6;
     if (n == 0) continue;
-    graph_count_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(g, d, need);
+    graph_count_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(g, d, need, multi);
     if (d > g.fd) add_launches(1);
   }
   OF_LAUNCH_CHECK("of_graph_count");
   return OF_OK;
 }
 
-extern "C" int of_graph_fill(const of_octree_levels* oct, int32_t D, const int32_t* need_off, int32_t* tap_tab,
-                             int32_t* tap_extra, uint8_t* node_type, int32_t* batch_id, void* stream) {
+extern "C" int of_graph_fill(const of_octree_levels* oct, int32_t D, const int32_t* need_off, const int32_t* multi_ord,
+                             int32_t n_multi, int32_t* tap_tab, int32_t* tap_extra, uint8_t* node_type,
+                             int32_t* batch_id, void* stream) {
   GraphCtx g;
   int rc = make_ctx(oct, D, g, "of_graph_fill");
   if (rc) return rc;
-  OF_REQUIRE(need_off && tap_tab && tap_extra, "of_graph_fill: null pointer");
+  OF_REQUIRE(need_off && multi_ord && tap_tab && tap_extra && n_multi >= 0, "of_graph_fill: bad arguments");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   for (int d = g.fd; d <= D; ++d) {
     const int64_t n = (int64_t)g.nnum[d] * 6;
     if (n == 0) continue;
-    graph_fill_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(g, d, need_off, tap_tab, tap_extra, node_type,
-                                                                  batch_id);
+    graph_fill_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(g, d, need_off, multi_ord, n_multi, tap_tab,
+                                                                  tap_extra, node_type, batch_id);
     if (d > g.fd) add_launches(1);
   }
   OF_LAUNCH_CHECK("of_graph_fill");

@@ -27,7 +27,7 @@ void add_launches(int n) { __atomic_fetch_add(&g_launches, (unsigned long long)n
 
 extern "C" unsigned long long of_launch_count(void) { return __atomic_load_n(&of::g_launches, __ATOMIC_RELAXED); }
 extern "C" const char* of_last_error(void) { return of::g_err; }
-extern "C" int of_version(void) { return 6; }
+extern "C" int of_version(void) { return 7; }
 extern "C" int of_abi_sizeof_gemm_args(void) { return (int)sizeof(of_gemm_args); }
 extern "C" int of_abi_sizeof_octree_levels(void) { return (int)sizeof(of_octree_levels); }
 extern "C" int of_num_sms(void) { return of::num_sms(); }

@@ -97,46 +97,46 @@ class DualOctree:
             self._keep += [keys, child, rank, scratch]
         self._levels = lv
         # ---- one tap table per graph depth ----
-        # Three phases so that the data-dependent sizes of ALL depths are fetched with two host synchronisations per
-        # octree (not ~3 per depth): (A) count + scan, sync 1 = neighbour-record words; (B) fill, multi-neighbour flags
-        # + scan, statistics segments, sync 2 = multi-slot and segment counts; (C) ordinal tables.
+        # Two phases so that the data-dependent sizes of ALL depths are fetched with two host synchronisations per
+        # octree (not ~3 per depth): (A) count + scans, sync 1 = neighbour words and multi-slot counts; (B) fill,
+        # statistics segments, sync 2 = segment counts.
         self.plan = {}
         self.graph = [dict() for _ in range(dep + 1)]
         depths = list(range(fd, dep + 1))
-        need_off, rows_of = {}, {}
+        scans, rows_of = {}, {}
         for D in depths:
             rows = int(lib.of_graph_rows(C.byref(lv), D))
             if rows < 0:
                 raise RuntimeError('of_graph_rows: ' + _lib.last_error())
             need = torch.empty(rows * N_DIR, dtype=torch.int32, device=dev)
-            check(lib.of_graph_count(C.byref(lv), D, ptr(need), stream()), 'of_graph_count')
-            need_off[D], rows_of[D] = ops.exclusive_scan_i32(need), rows
-        totals = torch.cat([need_off[D][-1:] for D in depths]).tolist()           # sync 1
+            multi = torch.empty(rows * N_DIR, dtype=torch.int32, device=dev)
+            check(lib.of_graph_count(C.byref(lv), D, ptr(need), ptr(multi), stream()), 'of_graph_count')
+            scans[D], rows_of[D] = (ops.exclusive_scan_i32(need), ops.exclusive_scan_i32(multi)), rows
+        totals = torch.cat([s[-1:] for D in depths for s in scans[D]]).tolist()   # sync 1
         pending = []
-        for D, total in zip(depths, totals):
-            rows = rows_of[D]
+        for i, D in enumerate(depths):
+            rows, (need_off, multi_ord) = rows_of[D], scans[D]
+            words, n_multi = totals[2 * i], totals[2 * i + 1]
             tab = torch.empty((rows, N_DIR), dtype=torch.int32, device=dev)
-            extra = torch.empty(max(int(total), 1), dtype=torch.int32, device=dev)
+            extra = torch.empty(n_multi + 1 + words, dtype=torch.int32, device=dev)
             ntype = torch.empty(rows, dtype=torch.uint8, device=dev)
             bid = torch.empty(rows, dtype=torch.int32, device=dev)
-            check(lib.of_graph_fill(C.byref(lv), D, ptr(need_off[D]), ptr(tab), ptr(extra), ptr(ntype), ptr(bid),
-                                    stream()), 'of_graph_fill')
+            check(lib.of_graph_fill(C.byref(lv), D, ptr(need_off), ptr(multi_ord), n_multi, ptr(tab), ptr(extra),
+                                    ptr(ntype), ptr(bid), stream()), 'of_graph_fill')
             hist = torch.zeros(self.batch_size, dtype=torch.int32, device=dev)
             check(lib.of_histogram_i32(ptr(bid), rows, self.batch_size, ptr(hist), stream()), 'of_histogram_i32')
             p = GraphPlan()
             p.depth, p.rows = D, rows
-            p.tap = ops.TapTable(tab, extra, N_DIR)
+            p.tap = ops.TapTable(tab, extra, N_DIR, n_multi)
             p.node_type, p.batch_id, p.rows_of_sample = ntype, bid, hist
             p.stat = ops.StatPlan(rows, self.batch_size, sample_id=bid, rows_of_sample=hist, defer=True)
-            pending += [p.tap.multi_prepare().long(), p.stat.pending_count().long()]
+            pending.append(p.stat.pending_count().long())
             p.leaf_base = int(self.lnum[fd:D].sum())          # rows of leaves coarser than D
             self.plan[D] = p
             self.graph[D] = _LazyGraph(self, D)
         counts = torch.cat(pending).tolist()                                      # sync 2
-        for i, D in enumerate(depths):
-            p = self.plan[D]
-            p.tap.multi_finish(counts[2 * i])
-            p.stat.finish(counts[2 * i + 1])
+        for D, n_seg in zip(depths, counts):
+            self.plan[D].stat.finish(n_seg)
         # ---- row maps of GraphDownsample / GraphUpsample (reference modules.py:409-428, 458-472) ----
         ar = lambda n: torch.arange(n, dtype=torch.int32, device=dev)  # noqa: E731
         for D in range(fd + 1, dep + 1):

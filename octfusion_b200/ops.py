@@ -43,18 +43,15 @@ def set_force_simt(flag: bool):
 
 
 class TapTable:
-    """Neighbour table of the tap-gather GEMM (see include/octfusion_b200.h).
-    tab/extra: record encoding (CUDA-core path).  tab_ord/multi_off: ordinal encoding of the multi-neighbour slots for
-    the tensor-core path (of_graph_multi_index); n_multi = number of such slots."""
-    __slots__ = ('tab', 'extra', 'taps', 'rows', 'tab_ord', 'multi_off', 'n_multi', '_type_blocks', '_scan')
+    """Neighbour table of the tap-gather GEMM (see include/octfusion_b200.h): tab [rows, taps] and the CSR lists `extra`
+    of its n_multi multi-neighbour slots (None when there is none)."""
+    __slots__ = ('tab', 'extra', 'taps', 'rows', 'n_multi', '_type_blocks')
 
-    def __init__(self, tab: torch.Tensor, extra, taps: int):
+    def __init__(self, tab: torch.Tensor, extra, taps: int, n_multi: int = 0):
         assert tab.dtype == torch.int32 and tab.is_contiguous()
-        self.tab, self.extra, self.taps = tab, extra, taps
+        self.tab, self.extra, self.taps, self.n_multi = tab, extra, taps, n_multi
         self.rows = tab.numel() // taps
-        self.tab_ord, self.multi_off, self.n_multi = tab, None, 0
         self._type_blocks = {}
-        self._scan = None
 
     def type_block(self, ntype, node_type):
         """bf16 [rows, 64] node-type K block of the tensor-core GEMM (graph constant, built once per ntype)."""
@@ -64,27 +61,6 @@ class TapTable:
                                           ptr(out), stream()), 'of_graph_type_block')
             self._type_blocks[ntype] = out
         return self._type_blocks[ntype]
-
-    def multi_prepare(self):
-        """flag + scan of the multi-neighbour slots; returns their count as a device scalar (no synchronisation)"""
-        slots = self.tab.numel()
-        flags = torch.empty(slots, dtype=torch.int32, device=self.tab.device)
-        check(lib.of_graph_multi_flags(ptr(self.tab), slots, ptr(flags), stream()), 'of_graph_multi_flags')
-        self._scan = exclusive_scan_i32(flags)
-        return self._scan[-1:]
-
-    def multi_finish(self, n_multi: int):
-        """build the ordinal-encoded table (once per graph) from multi_prepare's scan and its count"""
-        scan = self._scan
-        self._scan = None
-        self.n_multi = int(n_multi)
-        if self.n_multi == 0:
-            return self
-        self.tab_ord = torch.empty_like(self.tab)
-        self.multi_off = torch.empty(self.n_multi, dtype=torch.int32, device=self.tab.device)
-        check(lib.of_graph_multi_index(ptr(self.tab), ptr(self.extra), self.tab.numel(), ptr(scan), ptr(self.tab_ord),
-                                       ptr(self.multi_off), stream()), 'of_graph_multi_index')
-        return self
 
 
 class StatPlan:
@@ -266,17 +242,14 @@ def gather_gemm(a0, w: PreparedWeight, *, a1=None, tap: TapTable = None, in_rows
     g.reverse = _next_direction() if use_tc else 0
     if use_tc and w.ntype > 0 and tap is not None:
         g.nt_block = tap.type_block(w.ntype, node_type).data_ptr()
-    if tap is not None and use_tc:
-        g.tap_tab = tap.tab_ord.data_ptr()
-        if tap.n_multi > 0:
-            # slots with several (4..16) finer neighbours: their mean rows are built once per input tensor
-            aux = torch.empty((tap.n_multi, c0 + c1), dtype=act_dtype, device=a0.device)
-            check(lib.of_gather_mean_rows(a0.data_ptr(), a0.stride(0), c0, a1.data_ptr() if a1 is not None else None,
-                                          a1.stride(0) if a1 is not None else 0, c1, ptr(tap.extra), ptr(tap.multi_off),
-                                          tap.n_multi, dt(a0), ptr(aux), aux.stride(0), stream()), 'of_gather_mean_rows')
-            g.a_multi, g.ld_multi = aux.data_ptr(), aux.stride(0)
-    else:
-        g.tap_tab = tap.tab.data_ptr() if tap is not None else None
+    if use_tc and tap is not None and tap.n_multi > 0:
+        # slots with several (4..16) finer neighbours: their mean rows are built once per input tensor
+        aux = torch.empty((tap.n_multi, c0 + c1), dtype=act_dtype, device=a0.device)
+        check(lib.of_gather_mean_rows(a0.data_ptr(), a0.stride(0), c0, a1.data_ptr() if a1 is not None else None,
+                                      a1.stride(0) if a1 is not None else 0, c1, ptr(tap.extra), tap.n_multi, dt(a0),
+                                      ptr(aux), aux.stride(0), stream()), 'of_gather_mean_rows')
+        g.a_multi, g.ld_multi = aux.data_ptr(), aux.stride(0)
+    g.tap_tab = tap.tab.data_ptr() if tap is not None else None
     g.tap_extra = tap.extra.data_ptr() if (tap is not None and tap.extra is not None) else None
     g.in_rows = in_rows.data_ptr() if in_rows is not None else None
     g.taps = taps

@@ -36,6 +36,7 @@ def test_graph_invariants_full_size(doc):
     doc2 = product_doctree(B, 1000)
     for d in range(4, 7):
         assert torch.equal(doc.plan[d].tap.tab, doc2.plan[d].tap.tab)
+        assert torch.equal(doc.plan[d].tap.extra, doc2.plan[d].tap.extra)
         assert torch.equal(doc.plan[d].batch_id, doc2.plan[d].batch_id)
 
 

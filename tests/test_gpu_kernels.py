@@ -43,6 +43,30 @@ def test_graph_build_matches_oracle(batch, seed):
         assert bool((key[1:] >= key[:-1]).all())
 
 
+@pytest.mark.parametrize('batch,seed', [(1, 0), (2, 0), (3, 5)])
+def test_tap_table_encoding(batch, seed):
+    """the tap table decodes to the oracle's edge set by the header's rules: v >= 0 one row, -1 none, v <= -2 multi slot
+    o = -(v+2), numbered in slot order, whose rows are tap_extra[tap_extra[o] .. tap_extra[o+1])"""
+    dg, _ = oracle_doctree(batch, seed)
+    doc = product_doctree(batch, seed)
+    for d in range(4, 7):
+        tap = doc.plan[d].tap
+        tab, extra, n = tap.tab.cpu().long().flatten(), tap.extra.cpu().long(), tap.n_multi
+        off = extra[:n + 1]
+        assert int(off[0]) == n + 1 and int(off[-1]) == extra.numel(), 'offsets at depth %d' % d
+        cnt = off[1:] - off[:-1]
+        assert bool((cnt >= 2).all()), 'a multi slot with fewer than 2 rows at depth %d' % d   # offsets increase
+        multi = tab <= -2
+        assert torch.equal(-(tab[multi] + 2), torch.arange(n)), 'ordinals out of slot order at depth %d' % d
+        # the offsets tile tap_extra[n+1:], so the slots' rows follow one another in slot order
+        slot = torch.arange(tab.numel())
+        key = torch.cat([slot[tab >= 0], slot[multi].repeat_interleave(cnt)])
+        col = torch.cat([tab[tab >= 0], extra[n + 1:]])
+        a = R.edge_set({'edge_idx': torch.stack([key // 7, col]), 'edge_dir': key % 7})
+        b = R.edge_set(dg.graph[d])
+        assert torch.equal(a[0], b[0]) and torch.equal(a[1], b[1]), 'decoded edge set differs at depth %d' % d
+
+
 def test_scan_and_histogram():
     from octfusion_b200 import ops
     for n in (0, 1, 5, 2048, 2049, 1000003):

@@ -27,7 +27,7 @@ def test_library_matches_declared_abi():
     for name in declared:
         assert hasattr(lib, name), 'library does not export %s' % name
     assert declared == set(_lib.EXPORTED_SYMBOLS), declared ^ set(_lib.EXPORTED_SYMBOLS)
-    assert lib.of_version() == 6
+    assert lib.of_version() == 7
 
 
 def test_argument_validation_without_gpu():
