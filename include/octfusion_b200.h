@@ -379,6 +379,29 @@ int of_match_cost(const float* a, const float* b, int32_t batch, int32_t n, floa
  * of_match_cost (emd = cost / n) and cd [na, nb] as of_match_cost's cd, for xyz1 = a_i, xyz2 = b_j. */
 int of_emd_cd_pairwise(const float* a, int32_t na, const float* b, int32_t nb, int32_t n, float* cost, float* cd,
                        void* stream);
+/* Exact EMD (reference metrics/evaluation_metrics.py `emd_approx`, :35-52, which solves the fp32 distance matrix with
+ * scipy.optimize.linear_sum_assignment and averages the matched distances).  For a pair (x, y) of n points each:
+ *   d_ij = sqrt((dx*dx + dy*dy) + dz*dz) in fp32, every operation rounded on its own (d(x_i, y_j) == d(y_j, x_i));
+ *   s    = the smallest power of two >= the diagonal of the pair's joint bounding box (at least 2^-100), the squared
+ *          diagonal formed in fp64 from the fp32 extremes as (ex*ex + ey*ey) + ez*ez;  q = s 2^-24;
+ *   c_ij = rint(d_ij / q), an integer (ties to even);
+ *   emd  = (float)(C* q / n), formed in fp64, where C* is the optimal assignment cost of the integer matrix c.
+ * C* is unique, so emd is bit-reproducible whichever optimal assignment is found, and it lies within q/2 of the exact
+ * optimum of the fp32 matrix d (each c_ij q is within q/2 of d_ij); q scales with the pair, so this holds for
+ * unit-cube and world-scale clouds alike.  Solved by an auction with epsilon scaling on costs c (n + 1), one CTA per
+ * pair, no n^2 matrix in memory.  gap (int64, may be NULL) = P - D of the final prices, P the primal cost and D the
+ * dual bound, both in units of c / (n + 1); 0 <= gap <= n certifies optimality.
+ * status (int32, one per result): bits 0-3 = 0 solved, 1 round cap reached (a defect, never an input), 2 a coordinate
+ * is not finite, 3 the diagonal exceeds 2^62 (fp32 squares could overflow); bits 4-7 = epsilon phases run;
+ * bits 8-31 = bidding rounds over all phases (saturating).  Where bits 0-3 != 0 the result is NaN and the gap -1.
+ * Launches one kernel, synchronises nothing; 1 <= n <= OF_EMD_MAX_POINTS; results repeat bit for bit. */
+int of_emd_exact(const float* x, const float* y, int32_t batch, int32_t n, float* emd, int64_t* gap, int32_t* status,
+                 void* stream);
+/* all pairs: out, gap, status [na, nb] for (a_i, b_j), each entry equal to of_emd_exact of the pair.  symmetric != 0
+ * needs a == b and na == nb: only i < j is solved, the result is mirrored (d is exactly symmetric, so c and C* are)
+ * and the diagonal is 0 with status 0.  At most 2^31 - 2 pairs per call. */
+int of_emd_exact_pairwise(const float* a, int32_t na, const float* b, int32_t nb, int32_t n, int32_t symmetric,
+                          float* out, int64_t* gap, int32_t* status, void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * Meshes and metric point clouds.  Marching cubes replaces skimage.measure.marching_cubes(sdf, level) of export_mesh

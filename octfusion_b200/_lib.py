@@ -94,6 +94,8 @@ _PROTOS = {
     'of_chamfer_pairwise': (C.c_int, [_vp, _i32, _i32, _vp, _i32, _i32, _vp, _vp]),
     'of_match_cost': (C.c_int, [_vp, _vp, _i32, _i32, _vp, _vp, _vp]),
     'of_emd_cd_pairwise': (C.c_int, [_vp, _i32, _vp, _i32, _i32, _vp, _vp, _vp]),
+    'of_emd_exact': (C.c_int, [_vp, _vp, _i32, _i32, _vp, _vp, _vp, _vp]),
+    'of_emd_exact_pairwise': (C.c_int, [_vp, _i32, _vp, _i32, _i32, _i32, _vp, _vp, _vp, _vp]),
     'of_mc_count': (C.c_int, [_vp, _i32, _f32, _vp, _vp, _vp]),
     'of_mc_emit': (C.c_int, [_vp, _i32, _f32, _vp, _vp, _vp, _vp, _vp]),
     'of_mesh_bbox': (C.c_int, [_vp, _vp, _i32, _vp, _vp]),

@@ -13,7 +13,7 @@ CSRC = os.path.join(HERE, 'csrc')
 LIBDIR = os.path.join(HERE, 'lib')
 LIB = os.path.join(LIBDIR, 'liboctfusion_b200.so')
 SOURCES = ['runtime.cu', 'gemm_simt.cu', 'gemm_tc.cu', 'norm.cu', 'attention.cu', 'misc.cu', 'graph.cu', 'mpu.cu', 'metrics.cu',
-           'mesh.cu', 'points.cu', 'mesh_components.cu']
+           'emd_exact.cu', 'mesh.cu', 'points.cu', 'mesh_components.cu']
 NVCC_FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-O3', '-lineinfo', '-std=c++17',
               '-Xcompiler', '-fPIC', '--expt-relaxed-constexpr', '--extended-lambda']
 

@@ -1,23 +1,30 @@
 """Point-cloud shape metrics of the OctFusion evaluation on the GPU: MMD, COV and 1-NNA with Chamfer distance (CD)
-and approximate EMD.
+and EMD, approximate (the default) or exact (`accelerated_emd=False`).
 
 Drop-in for reference metrics/evaluation_metrics.py (and the `nn_distance` / `match_cost` functions of
 metrics/pytorch_structural_losses): the names, argument order, orientation and dict keys are the reference's, so its
 callers can swap modules.  The all-pairs distance matrices, the O(N^2 P^2) part, are computed by the kernels of
-csrc/metrics.cu, one launch per matrix; the O(N^2) reductions over finished matrices (min, unique, top-k) are torch
-ops on the device.
+csrc/metrics.cu and csrc/emd_exact.cu, one launch per matrix; the O(N^2) reductions over finished matrices (min,
+unique, top-k) are torch ops on the device.
 
 Inputs are contiguous fp32 CUDA tensors [N, P, 3]; anything else raises (there is no CPU path).  `batch_size`
 arguments are accepted for signature compatibility and ignored: every matrix is computed in one launch without
 copying any cloud.  Results carry no gradient.
+
+The reference has two EMDs.  `accelerated_emd=True` (the default everywhere here) is the approximate match cost of
+pytorch_structural_losses (`emd_approx_cuda`).  `accelerated_emd=False` is the exact EMD that the reference's
+`emd_approx` computes with scipy's linear_sum_assignment, and that its metrics fall back to when the structural-loss
+extension is not importable; CD is the same in both arms.  The exact EMD is the optimal assignment cost of distances
+quantised to q = 2^-24 times the pair's bounding-box scale (include/octfusion_b200.h, of_emd_exact): within q/2 of
+the optimum of the fp32 distance matrix, and bit-reproducible.
 """
 from __future__ import annotations
 import torch
 
 from ._lib import lib, ptr, stream, check, EMD_MAX_POINTS, CD_PAIRWISE_MAX_POINTS
 
-__all__ = ['nn_distance', 'match_cost', 'paired_emd_cd', 'EMD_CD', 'pairwise_cd', 'pairwise_emd_cd', 'lgan_mmd_cov',
-           'knn', 'compute_cov_mmd', 'compute_1_nna', 'compute_all_metrics']
+__all__ = ['nn_distance', 'match_cost', 'paired_emd_cd', 'emd_approx', 'emd_exact', 'pairwise_emd_exact', 'EMD_CD',
+           'pairwise_cd', 'pairwise_emd_cd', 'lgan_mmd_cov', 'knn', 'compute_cov_mmd', 'compute_1_nna', 'compute_all_metrics']
 
 
 def _clouds(x, name):
@@ -38,14 +45,13 @@ def _same_device(x, y):
     torch.cuda.set_device(x.device)
 
 
-def _equal_sizes(x, y):
+def _equal_sizes(x, y, what='approximate EMD'):
     n = x.shape[1]
     if y.shape[1] != n:
-        raise ValueError('octfusion_b200.metrics: approximate EMD needs clouds of equal size, got %d and %d'
-                         % (n, y.shape[1]))
+        raise ValueError('octfusion_b200.metrics: %s needs clouds of equal size, got %d and %d' % (what, n, y.shape[1]))
     if n > EMD_MAX_POINTS:
-        raise ValueError('octfusion_b200.metrics: approximate EMD supports up to %d points per cloud, got %d'
-                         % (EMD_MAX_POINTS, n))
+        raise ValueError('octfusion_b200.metrics: %s supports up to %d points per cloud, got %d'
+                         % (what, EMD_MAX_POINTS, n))
     return n
 
 
@@ -88,12 +94,76 @@ def paired_emd_cd(x, y):
     return cd, cost / x.shape[1]
 
 
+_EXACT_FAILURES = {1: (RuntimeError, 'the auction reached its round cap (a solver defect; please report the input)'),
+                   2: (ValueError, 'a coordinate is not finite'),
+                   3: (ValueError, 'the bounding-box diagonal exceeds 2^62, beyond fp32 squared distances')}
+
+
+def _check_exact(status, what):
+    """raise on the first failed pair; reading the statuses is the call's one host synchronisation"""
+    code = status.cpu() & 15
+    if code.any():
+        idx = tuple(int(i) for i in torch.nonzero(code)[0])
+        exc, why = _EXACT_FAILURES.get(int(code[idx]), (RuntimeError, 'status %d' % int(code[idx])))
+        raise exc('octfusion_b200.metrics: %s: pair %s: %s' % (what, idx[0] if len(idx) == 1 else idx, why))
+
+
 @torch.no_grad()
-def EMD_CD(sample_pcs, ref_pcs, batch_size=None, reduced=True):
-    """{'MMD-CD', 'MMD-EMD'} of the matched pairs (sample_pcs[i], ref_pcs[i]) (reference EMD_CD, accelerated arms)."""
+def emd_exact(x, y, details=False):
+    """[B] exact EMD of (x[i], y[i]): the mean matched distance of an optimal assignment (of_emd_exact).  With
+    details=True returns (emd, gap, status): gap [B] int64 is the primal-dual gap of the final auction prices
+    (0 <= gap <= n certifies optimality), status [B] int32 the solver's status word (bits 4-7 phases, 8-31 rounds)."""
+    _clouds(x, 'x'); _clouds(y, 'y'); _same_device(x, y)
+    if x.shape[0] != y.shape[0]:
+        raise ValueError('octfusion_b200.metrics: batch sizes differ (%d, %d)' % (x.shape[0], y.shape[0]))
+    n = _equal_sizes(x, y, 'exact EMD')
+    b = x.shape[0]
+    emd = torch.empty(b, device=x.device)
+    gap = torch.empty(b, dtype=torch.int64, device=x.device)
+    status = torch.zeros(b, dtype=torch.int32, device=x.device)
+    check(lib.of_emd_exact(ptr(x), ptr(y), b, n, ptr(emd), ptr(gap), ptr(status), stream()), 'emd_exact')
+    _check_exact(status, 'emd_exact')
+    return (emd, gap, status) if details else emd
+
+
+@torch.no_grad()
+def emd_approx(x, y):
+    """[B] exact EMD of (x[i], y[i]) under the reference's name: reference `emd_approx`, despite the name, solves the
+    distance matrix exactly (metrics/evaluation_metrics.py:35-52)."""
+    return emd_exact(x, y)
+
+
+@torch.no_grad()
+def pairwise_emd_exact(a, b, details=False):
+    """emd [Na, Nb]: exact EMD of every pair (a[i], b[j]), each entry equal to emd_exact of the pair.  When `a is b`
+    only i < j is solved and mirrored (the exact EMD is symmetric bit for bit) and the diagonal is 0.  details=True
+    returns (emd, gap, status) as emd_exact does."""
+    _clouds(a, 'a'); _clouds(b, 'b'); _same_device(a, b)
+    n = _equal_sizes(a, b, 'exact EMD')
+    emd = torch.empty(a.shape[0], b.shape[0], device=a.device)
+    gap = torch.empty(a.shape[0], b.shape[0], dtype=torch.int64, device=a.device)
+    status = torch.zeros(a.shape[0], b.shape[0], dtype=torch.int32, device=a.device)
+    check(lib.of_emd_exact_pairwise(ptr(a), a.shape[0], ptr(b), b.shape[0], n, 1 if a is b else 0, ptr(emd), ptr(gap),
+                                    ptr(status), stream()), 'pairwise_emd_exact')
+    _check_exact(status, 'pairwise_emd_exact')
+    return (emd, gap, status) if details else emd
+
+
+@torch.no_grad()
+def EMD_CD(sample_pcs, ref_pcs, batch_size=None, reduced=True, accelerated_emd=True):
+    """{'MMD-CD', 'MMD-EMD'} of the matched pairs (sample_pcs[i], ref_pcs[i]) (reference EMD_CD).  accelerated_emd
+    selects the approximate EMD (True, fused with the CD) or the exact one (False, CD from nn_distance)."""
     if sample_pcs.shape[0] != ref_pcs.shape[0]:
         raise ValueError('octfusion_b200.metrics: REF:%d SMP:%d' % (ref_pcs.shape[0], sample_pcs.shape[0]))
-    cd, emd = paired_emd_cd(sample_pcs, ref_pcs)
+    if accelerated_emd:
+        cd, emd = paired_emd_cd(sample_pcs, ref_pcs)
+    else:
+        emd = emd_exact(sample_pcs, ref_pcs)
+        cd = torch.empty_like(emd)
+        d1 = torch.empty(sample_pcs.shape[:2], device=emd.device)
+        d2 = torch.empty(ref_pcs.shape[:2], device=emd.device)
+        check(lib.of_nn_distance(ptr(sample_pcs), ptr(ref_pcs), sample_pcs.shape[0], sample_pcs.shape[1],
+                                 ref_pcs.shape[1], ptr(d1), ptr(d2), ptr(cd), stream()), 'EMD_CD')
     if reduced:
         cd, emd = cd.mean(), emd.mean()
     return {'MMD-CD': cd, 'MMD-EMD': emd}
@@ -112,9 +182,12 @@ def pairwise_cd(a, b, batch_size=None):
 
 
 @torch.no_grad()
-def pairwise_emd_cd(a, b, batch_size=None):
+def pairwise_emd_cd(a, b, batch_size=None, accelerated_emd=True):
     """(cd [Na, Nb], emd [Na, Nb]) of every pair with a[i] as the first cloud (reference `_pairwise_EMD_CD_`).
-    Approximate EMD is not symmetric: a matrix of a set against itself is computed in full, not mirrored."""
+    Approximate EMD is not symmetric: a matrix of a set against itself is computed in full, not mirrored.  With
+    accelerated_emd=False the EMD is exact (pairwise_emd_exact, mirrored when `a is b`) and CD is pairwise_cd."""
+    if not accelerated_emd:
+        return pairwise_cd(a, b), pairwise_emd_exact(a, b)
     _clouds(a, 'a'); _clouds(b, 'b'); _same_device(a, b)
     n = _equal_sizes(a, b)
     cost = torch.empty(a.shape[0], b.shape[0], device=a.device)
@@ -176,23 +249,26 @@ def _one_nna(m_rs, m_rr, m_ss):
 
 
 @torch.no_grad()
-def compute_cov_mmd(sample_pcs, ref_pcs, batch_size=None):
+def compute_cov_mmd(sample_pcs, ref_pcs, batch_size=None, accelerated_emd=True):
     """lgan_mmd / lgan_cov / lgan_mmd_smp with CD and EMD; the matrix is reference x sample, transposed to
-    [N_sample, N_ref] (reference compute_cov_mmd)."""
-    return _cov_mmd(*pairwise_emd_cd(ref_pcs, sample_pcs))
+    [N_sample, N_ref] (reference compute_cov_mmd).  accelerated_emd=False: exact EMD."""
+    return _cov_mmd(*pairwise_emd_cd(ref_pcs, sample_pcs, accelerated_emd=accelerated_emd))
 
 
 @torch.no_grad()
-def compute_1_nna(sample_pcs, ref_pcs, batch_size=None):
-    """1-NN-{CD,EMD}-{acc_t,acc_f,acc} (reference compute_1_nna)."""
-    return _one_nna(pairwise_emd_cd(ref_pcs, sample_pcs), pairwise_emd_cd(ref_pcs, ref_pcs),
-                    pairwise_emd_cd(sample_pcs, sample_pcs))
+def compute_1_nna(sample_pcs, ref_pcs, batch_size=None, accelerated_emd=True):
+    """1-NN-{CD,EMD}-{acc_t,acc_f,acc} (reference compute_1_nna).  accelerated_emd=False: exact EMD."""
+    return _one_nna(pairwise_emd_cd(ref_pcs, sample_pcs, accelerated_emd=accelerated_emd),
+                    pairwise_emd_cd(ref_pcs, ref_pcs, accelerated_emd=accelerated_emd),
+                    pairwise_emd_cd(sample_pcs, sample_pcs, accelerated_emd=accelerated_emd))
 
 
 @torch.no_grad()
-def compute_all_metrics(sample_pcs, ref_pcs, batch_size=None):
-    """compute_cov_mmd and compute_1_nna in one call; the reference x sample matrices are computed once."""
-    m_rs = pairwise_emd_cd(ref_pcs, sample_pcs)
+def compute_all_metrics(sample_pcs, ref_pcs, batch_size=None, accelerated_emd=True):
+    """compute_cov_mmd and compute_1_nna in one call; the reference x sample matrices are computed once.
+    accelerated_emd=False: exact EMD."""
+    m_rs = pairwise_emd_cd(ref_pcs, sample_pcs, accelerated_emd=accelerated_emd)
     out = _cov_mmd(*m_rs)
-    out.update(_one_nna(m_rs, pairwise_emd_cd(ref_pcs, ref_pcs), pairwise_emd_cd(sample_pcs, sample_pcs)))
+    out.update(_one_nna(m_rs, pairwise_emd_cd(ref_pcs, ref_pcs, accelerated_emd=accelerated_emd),
+                        pairwise_emd_cd(sample_pcs, sample_pcs, accelerated_emd=accelerated_emd)))
     return out
